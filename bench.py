@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- warp + multiband-blend throughput of the B200 compositing path (BASELINE.json metric).
+"""bench.py -- warp + multiband-blend throughput of the H100 compositing path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg2]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg2] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic frames for a fixed rig: fused warp of
 every image (+ validity mask), Gaussian/weight pyramids, per-band weighted accumulate + normalise + collapse,
@@ -13,8 +13,10 @@ and pano column strips per rank, one grouped NCCL send/recv of the per-band part
 
 Prints ONE JSON line (rank 0).  `value` is device-resident throughput (inputs already in HBM, CUDA events on
 the launching stream); `e2e` goes through the public API with pinned HOST buffers, host<->device copies inside
-the timed region; `roofline` is the dominant kernel against the measured HBM copy bandwidth; `cpu_baseline`
-is the reference's own cv2 path (oracle/cv_path.py) timed on this box's host cores.
+the timed region; `roofline` is the dominant kernel against the HBM bandwidth; `cpu_baseline` is the reference's
+own cv2 path (oracle/cv_path.py) timed on the host's cores.  `--dump-outputs DIR` writes what the last timed step
+computed (a fixed sample of the panorama and its mask, see dump_outputs) for comparing two builds output for output; it
+covers the single-panorama path of `--impl ours` (N = 1, or rank 0 with --replicas), not the sharded or reference arm.
 """
 import argparse
 import ctypes as C
@@ -144,18 +146,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(kernel):
-    """DRAM bytes per launch of `kernel` from the committed ncu capture, if one exists for this round."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get(kernel)
-        except Exception:  # noqa: BLE001
-            return None
-    return None
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 SCALE_DOWN = 1  # --scale-down (debug dry runs only; recorded in config, never a reportable number)
@@ -214,6 +205,26 @@ def compare_results(pano, mask, ref_pano, ref_mask):
     mask_diff = int(np.count_nonzero(mask != ref_mask))
     return {"differing": differing, "max_abs": max_abs, "mask_differing": mask_diff, "values": int(pano.size),
             "against": "the reference's cv2 path on the same inputs (oracle/cv_path.py), whole panorama"}
+
+
+DUMP_PIXELS = 2_000_000  # sampled panorama pixels: 24 MB of colour, 8 MB of mask, 16 MB of indices
+
+
+def dump_outputs(out_dir, pano, mask):
+    """Write what the timed path hands its caller -- the uint8 panorama and its mask -- for comparing two builds.
+    A panorama is larger than the 64 MB these files may take, so a fixed sample of pixels is written, drawn with
+    seed 0 from the panorama's shape alone: pano.npy (k x 3 float32), mask.npy (k float32), pixel_index.npy (k
+    float64, row-major flat indices) and pano_shape.npy (float64 [rows, cols])."""
+    os.makedirs(out_dir, exist_ok=True)
+    h, w = mask.shape
+    if h * w <= DUMP_PIXELS:
+        idx = np.arange(h * w)
+    else:
+        idx = np.unique(np.random.default_rng(0).integers(0, h * w, DUMP_PIXELS))
+    np.save(os.path.join(out_dir, "pano.npy"), np.ascontiguousarray(pano).reshape(-1, 3)[idx].astype(np.float32))
+    np.save(os.path.join(out_dir, "mask.npy"), np.ascontiguousarray(mask).reshape(-1)[idx].astype(np.float32))
+    np.save(os.path.join(out_dir, "pixel_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "pano_shape.npy"), np.array([h, w], np.float64))
 
 
 def cpu_baseline_block(cfg, imgs, gpu_pano=None, gpu_mask=None, budget_s=100.0):
@@ -385,8 +396,8 @@ def run_ours(args, rank, local_rank, world):
             c2.run()
         c2.sync()
         extra.append(c2)
-    single_ms, launches = comp.time(min(args.steps, 20), flush_l2=args.flush_l2)  # one batch at a time + per-kernel times
-    single_ms /= min(args.steps, 20)
+    single_ms, launches = comp.time(args.steps, flush_l2=args.flush_l2)  # one batch at a time + per-kernel times
+    single_ms /= args.steps
     dist.barrier()
     sampler = ClockSampler(local_rank)
     sampler.start()
@@ -400,6 +411,9 @@ def run_ours(args, rank, local_rank, world):
     for c2 in extra:
         c2.sync()
     clocks = sampler.result()
+    if args.dump_outputs and rank == 0:  # the compositor that ran the last timed step (steps are dealt round-robin)
+        last = ([comp] + extra)[(args.steps - 1) % (1 + len(extra))]
+        dump_outputs(args.dump_outputs, *last.download())
     dist.barrier()
     worst_ms = dist.max(total_ms)
     total_mpix = dist.sum(mpix_rank)
@@ -414,7 +428,7 @@ def run_ours(args, rank, local_rank, world):
     achieved = per_launch_bytes[k_dom] / (dom_ms * 1e-3) / 1e9
     roofline = {
         "bound": "hbm", "kernel": dom_name, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-        "traffic": ncu_traffic(dom_name), "peak_source": peak_src, "algorithmic_bytes": per_launch_bytes[k_dom],
+        "peak_source": peak_src, "algorithmic_bytes": per_launch_bytes[k_dom],
         "kernel_ms": dom_ms,
         "whole_step": {"algorithmic_bytes": total_bytes, "achieved": total_bytes / (total_ms / args.steps * 1e-3) / 1e9,
                        "frac": total_bytes / (total_ms / args.steps * 1e-3) / 1e9 / peak},
@@ -444,7 +458,7 @@ def run_ours(args, rank, local_rank, world):
     for _ in range(3):
         e2e_step()
     dist.barrier()
-    e2e_steps = max(4, min(args.steps, 40))
+    e2e_steps = args.steps
     t0 = time.perf_counter()
     for _ in range(3):
         e2e_step()
@@ -501,7 +515,7 @@ def run_ours(args, rank, local_rank, world):
                 "num_bands": comp.num_bands, "plan_ms": round(plan_ms, 2),
                 "batches_in_flight": args.inflight, "one_batch_at_a_time_ms_per_step": round(single_ms, 4),
                 "l2": "L2 flushed between steps" if args.flush_l2 else
-                      f"no flush: a step streams {total_bytes / 1e6:.0f} MB, inputs {n * src_bytes / 1e6:.0f} MB > 126 MB L2",
+                      f"no flush: a step streams {total_bytes / 1e6:.0f} MB, inputs {n * src_bytes / 1e6:.0f} MB > 50 MB L2",
                 "parallelism": "1 GPU" if world == 1 else f"{world} GPUs, one independent {n}-image ring per GPU (no collective)",
                 "timed": "plan (roi detection, trig tables, buffers) built once outside the timed region; a step = warp + pyramids + collapse kernels",
                 "source_layout": ("one word per pixel (r | g<<8 | b<<16): every upload is followed by a repack kernel on the copy stream, outside "
@@ -597,7 +611,7 @@ def run_sharded(args, rank, local_rank, world):
     for _ in range(3):
         e2e_step()
     dist.barrier()
-    e2e_steps = max(4, min(args.steps, 40))
+    e2e_steps = args.steps
     t0 = time.perf_counter()
     for _ in range(e2e_steps):
         e2e_step()
@@ -679,7 +693,7 @@ def run_sharded(args, rank, local_rank, world):
                 "parallelism": f"{world} GPUs: image blocks per rank, pano {'row' if rows else 'column'} strips per rank; the partial sums that cross strip "
                                f"boundaries go to the owner's memory over NVLink (copy engine + flags; SB_PEER=0: grouped NCCL send/recv) on a "
                                f"communication stream, overlapped with the kernels ({slab_total / 1e6:.1f} MB per step in total)",
-                "l2": f"no flush: each rank streams its {per_gpu * src_bytes / 1e6:.0f} MB of sources every step (> 126 MB L2)",
+                "l2": f"no flush: each rank streams its {per_gpu * src_bytes / 1e6:.0f} MB of sources every step (> 50 MB L2)",
                 "timed": ("plan built once; a step = warp + distance-transform weights + partial sums + exchange + normalise of the own strip" if grid else
                           "plan built once; a step = warp + pyramids + partial sums + exchange (level-0 slabs leave after the first pyrDown) + collapse of the own strip"),
                 "like_for_like_n1": like_for_like,
@@ -690,7 +704,7 @@ def run_sharded(args, rank, local_rank, world):
                     "api": "stitching_b200.Compositor(rank, world).upload/run/download per rank, pinned host buffers"},
             "gpu_launches": int(launches1 - launches0),
             "roofline": {"bound": "hbm", "kernel": None, "achieved": None, "peak": measured_peak_gbs()[0], "unit": "GB/s", "frac": None,
-                         "traffic": None, "note": "per-kernel roofline is reported at N = 1", "launches_ms_rank0": {k: round(v, 4) for k, v in launches}},
+                         "note": "per-kernel roofline is reported at N = 1", "launches_ms_rank0": {k: round(v, 4) for k, v in launches}},
             "cpu_baseline": None, "parity": parity,
             "result_checksum": int(pano[::97, ::89].astype(np.uint64).sum()),
         }
@@ -715,11 +729,18 @@ def main():
     ap.add_argument("--replicas", action="store_true", help="N > 1: one independent panorama per GPU instead of one sharded panorama")
     ap.add_argument("--extras", action="store_true", help="also fuse exposure gains and seam masks into the step (SURVEY 8f f1, f2)")
     ap.add_argument("--scale-down", type=int, default=1, help="debug: shrink the workload (not a valid measurement)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write a fixed sample of the last timed step's panorama and mask to DIR/*.npy; --impl ours with one "
+                         "panorama per GPU only (--gpus 1, or --replicas: rank 0's), not the sharded or the reference arm")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     global SCALE_DOWN
     SCALE_DOWN = args.scale_down
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank, local_rank, world = dist_env()
+    if args.dump_outputs and (args.impl == "reference" or (world > 1 and not args.replicas)):
+        ap.error("--dump-outputs is available for --impl ours on one panorama per GPU")
     if args.impl == "reference":
         run_reference(args, rank, world)
     elif world > 1 and not args.replicas:

@@ -1,5 +1,5 @@
 /*
- * stitch_b200.h -- C ABI of libstitch_b200.so: the B200-native (sm_100a) compositing hot path of
+ * stitch_b200.h -- C ABI of libstitch_b200.so: the H100-native (sm_90a) compositing hot path of
  * OpenStitching/stitching, i.e. what stitching/warper.py and stitching/blender.py reach in OpenCV.
  *
  * Conventions
@@ -9,7 +9,7 @@
  *     return except inside opaque handles.  Device memory is owned by the library.
  *   - images are uint8 HxWx3 interleaved with a row pitch in BYTES; masks are uint8 HxW.
  *   - K and R are row-major float32 3x3 (warper.py:84-94 get_K, camera.R).
- *   - there is NO CPU fallback: without a usable sm_100 device every compute entry fails with
+ *   - there is NO CPU fallback: without a usable sm_90 device every compute entry fails with
  *     SB_ERR_NO_DEVICE.
  *
  * Each entry cites the reference interface it replaces (file:line in OpenStitching/stitching v0.7.0).
@@ -29,7 +29,7 @@ extern "C" {
 typedef enum {
     SB_OK = 0,
     SB_ERR_INVALID = -1,   /* bad argument (what cv2 would assert on) */
-    SB_ERR_NO_DEVICE = -2, /* no CUDA device / not sm_100 */
+    SB_ERR_NO_DEVICE = -2, /* no CUDA device / not sm_90 */
     SB_ERR_CUDA = -3,      /* CUDA runtime failure, see sb_last_error */
     SB_ERR_STATE = -4,     /* call order violation (feed before prepare, blend twice, ...) */
     SB_ERR_NOMEM = -5,

@@ -1,4 +1,4 @@
-"""stitching_b200 -- the compositing hot path of OpenStitching/stitching on NVIDIA B200 (sm_100a).
+"""stitching_b200 -- the compositing hot path of OpenStitching/stitching on NVIDIA H100 (sm_90a).
 
 Drop-in replacements for `stitching.warper.Warper`, `stitching.blender.Blender` and `SeamFinder.resize` (same
 interface) backed by hand-written CUDA kernels behind a C ABI (include/stitch_b200.h), plus a fused `Compositor`.
@@ -19,12 +19,12 @@ _installed = {}
 
 
 def install(stitching_module=None):
-    """Route `stitching.Stitcher` (and cropper / seam finder / verbose callers) through the B200 classes.
+    """Route `stitching.Stitcher` (and cropper / seam finder / verbose callers) through the GPU classes.
 
     The reference modules bind the class names at import time (`from .warper import Warper` in
     stitcher.py, cropper.py, seam_finder.py, verbose.py), so the names are patched in each of them.  A reference
     module that cannot be imported is reported with a StitchingWarning (the pipeline would otherwise run half on cv2
-    and half on the B200 classes without a sign); any other failure propagates.
+    and half on the GPU classes without a sign); any other failure propagates.
     """
     import importlib
     import warnings
@@ -78,7 +78,7 @@ def install(stitching_module=None):
 
 def __getattr__(name):
     """`stitching_b200.Stitcher` / `stitching_b200.AffineStitcher` (stitching/__init__.py:1): the reference's pipeline
-    classes -- same DEFAULT_SETTINGS, same CLI -- running on the B200 classes.  They live in the reference package
+    classes -- same DEFAULT_SETTINGS, same CLI -- running on the GPU classes.  They live in the reference package
     (registration, seam estimation, cropping ... are its control plane); install() routes their hot path here."""
     if name in ("Stitcher", "AffineStitcher"):
         return getattr(install(), name)

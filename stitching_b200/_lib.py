@@ -1,6 +1,6 @@
 """ctypes binding of libstitch_b200.so (include/stitch_b200.h).
 
-There is no CPU fallback: if the CUDA library is missing or no sm_100 device is usable, importing the
+There is no CPU fallback: if the CUDA library is missing or no sm_90 device (H100) is usable, importing the
 binding works but the first call raises.  The library is built in-tree by `make -C stitching_b200/csrc`
 (or `__graft_entry__.build()`).
 """

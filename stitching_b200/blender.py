@@ -1,8 +1,8 @@
-"""B200 drop-in for stitching.blender.Blender (reference: stitching/blender.py:5-56).
+"""GPU drop-in for stitching.blender.Blender (reference: stitching/blender.py:5-56).
 
 prepare / feed / blend keep their signatures and return types.  feed() uploads and records the image;
 the arithmetic of cv.detail_MultiBandBlender / FeatherBlender / Blender(NO) runs in blend() as one batch
-of sm_100a kernels that applies the feeds in call order (bit-identical to eager accumulation).
+of sm_90a kernels that applies the feeds in call order (bit-identical to eager accumulation).
 """
 import ctypes as C
 
@@ -18,7 +18,8 @@ class _NativeBlender:
     def __init__(self, kind, num_bands=0, sharpness=0.0):
         self.kind = kind
         self.sharpness = float(sharpness)
-        self._h = _lib.lib().sb_blender_create(_lib.BLEND_KINDS[kind], int(num_bands), C.c_float(sharpness))
+        self._L = _lib.lib()  # the handle is destroyed by the library that created it, whichever is bound later
+        self._h = self._L.sb_blender_create(_lib.BLEND_KINDS[kind], int(num_bands), C.c_float(sharpness))
         if not self._h:
             _lib.check(-1, "sb_blender_create")
         self.roi = None
@@ -99,7 +100,7 @@ class _NativeBlender:
 
     def close(self):
         if self._h:
-            _lib.lib().sb_blender_destroy(self._h)
+            self._L.sb_blender_destroy(self._h)
             self._h = None
 
     def __del__(self):

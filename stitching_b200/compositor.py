@@ -1,4 +1,4 @@
-"""Fused warp + blend on one B200 with every intermediate resident in HBM (sb_compositor_* in the C ABI).
+"""Fused warp + blend on one GPU with every intermediate resident in HBM (sb_compositor_* in the C ABI).
 
 Equivalent to running, for a fixed rig, stitcher.py:178-189 (Warper.warp_images / create_and_warp_masks /
 warp_rois at final resolution) and stitcher.py:241-259 (Blender.prepare / feed / blend) -- with the warped
@@ -36,7 +36,7 @@ class Compositor:
         if n == 0 or len(sizes) != n:
             raise StitchingError("Compositor needs one size per camera")
         if warper_type not in _lib.WARP_TYPES:
-            raise StitchingError(f"warper type '{warper_type}' is not on the B200 path")
+            raise StitchingError(f"warper type '{warper_type}' is not on the GPU path")
         if blender_type not in _lib.BLEND_KINDS:
             raise StitchingError(f"unknown blender type '{blender_type}'")
         self.n = n
@@ -51,7 +51,7 @@ class Compositor:
         rig = _lib.Rig(n, _lib.WARP_TYPES[warper_type], np.float32(self.scale), _lib.BLEND_KINDS[blender_type],
                        np.float32(blend_strength), self._w, self._h, self._K.ctypes.data_as(_lib.c_float_p),
                        self._R.ctypes.data_as(_lib.c_float_p), 0)
-        L = _lib.lib()
+        L = self._L = _lib.lib()  # close() releases through the library that created the compositor
         self.rank, self.world = int(rank), int(world)
         if self.world > 1:
             self._c = L.sb_compositor_create_sharded(C.byref(rig), self.rank, self.world)
@@ -185,7 +185,7 @@ class Compositor:
     def pinned_empty(self, shape):
         """uint8 ndarray in page-locked host memory (freed with the compositor)."""
         nbytes = int(np.prod(shape))
-        p = _lib.lib().sb_host_alloc(nbytes)
+        p = self._L.sb_host_alloc(nbytes)
         if not p:
             _lib.check(-5, "sb_host_alloc")
         self._pinned.append(p)
@@ -222,10 +222,10 @@ class Compositor:
 
     def close(self):
         if getattr(self, "_c", None):
-            _lib.lib().sb_compositor_destroy(self._c)  # synchronises all its streams first
+            self._L.sb_compositor_destroy(self._c)  # synchronises all its streams first
             self._c = None
             for p in self._pinned:
-                _lib.lib().sb_host_free(p)
+                self._L.sb_host_free(p)
             self._pinned = []
 
     def __del__(self):

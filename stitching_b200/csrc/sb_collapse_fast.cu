@@ -1,7 +1,7 @@
 // sb_collapse_fast.cu -- instruction-lean version of the per-level multiband kernel, all levels.
 //
 // Same arithmetic as k_collapse_gather (sb_blend.cu; see there for the reference call chain
-// stitching/blender.py:41,46 -> MultiBandBlender::feed / ::blend), reorganised for the B200 SM, where the
+// stitching/blender.py:41,46 -> MultiBandBlender::feed / ::blend), reorganised for an issue-bound SM, where the
 // profile showed the kernel to be issue-bound rather than HBM-bound:
 //   * one thread per 2x2 quad: the four pixels share the 3x3 neighbourhood of the coarser level, so each pyrUp
 //     (of the image's G_{l+1} and of the collapsed C_{l+1}) is 9 taps per quad, evaluated through shared column sums;

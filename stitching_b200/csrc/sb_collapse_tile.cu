@@ -6,7 +6,7 @@
 // then n = (short)trunc(acc / (wsum + 1e-5)), C_l = sat16(pyrUp(C_{l+1}) + n), and at level 0 mask / |.| / uint8.
 //
 // What changed against k_collapse_fast is where the operands come from and how often they are touched.  The profile of
-// k_collapse_fast (profiles/ncu_r02_a_*) shows 845 warp instructions per quad at level 0: 340 in the final pyrUp +
+// k_collapse_fast shows 845 warp instructions per quad at level 0: 340 in the final pyrUp +
 // store, ~190 per covering image, mostly address arithmetic, bounds tests and 9 + 27 scattered global taps per thread.
 // Here a CTA owns a 64x16 tile (one thread per 2x2 quad) and stages every window the tile needs in shared memory with
 // asynchronous 16-byte copies (cp.async / LDGSTS, zero fill outside the source, the next image's windows in flight
@@ -20,10 +20,8 @@
 // collapse add and |.| / min run on two 16-bit lanes per word (VIADD.16x2, VIMNMX.S16x2) with exact integer forms
 // for the weight sums 0, 1 and 2 that make up almost all of a panorama.
 //
-// (The first version staged the windows with the tensor copy engine, cp.async.bulk.tensor / UTMALDG.  On this pool's
-// B200 boxes every tensor-map instruction -- the CUDA programming guide's own sample included -- ends in "illegal
-// instruction", while the 1-D bulk copy works: tests/tools/tma_*.cu, profiles/tma_probe_r02.md.  The staging therefore
-// uses cp.async; sb_tma.cuh keeps the wrappers.)
+// (The first version staged the windows with the tensor copy engine, cp.async.bulk.tensor / UTMALDG.  The staging
+// uses cp.async; sb_tma.cuh keeps the tensor-map wrappers.)
 //
 // Scope: byte-fed images, uint8 image + mask output, whole levels or a rank's strip of one (multi-GPU: the region may start
 // anywhere even; the tile grid starts at the 64-column boundary at or left of it and quads left of the region are idle).
@@ -544,8 +542,8 @@ bool collapse_tile_enabled()
 
 int launch_collapse_tile(const CollapseArgs &A, int l, int nb, cudaStream_t s)
 {
-    // levels 0 and 1 only: from level 2 on the per-tile staging overhead outweighs what it saves (measured on B200:
-    // level 2 0.040 ms against 0.038 ms for k_collapse_fast, level 3 0.018 against 0.017; SB_TILE_MAXL overrides)
+    // levels 0 and 1 only: from level 2 on the levels are small and the per-tile staging overhead outweighs what it
+    // saves (SB_TILE_MAXL overrides)
     static const int max_level = [] {
         const char *e = getenv("SB_TILE_MAXL");
         return e ? atoi(e) : 1;

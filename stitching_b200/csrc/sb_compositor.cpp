@@ -906,7 +906,7 @@ int sb_compositor_time(sb_compositor *c, int iters, int flush_l2, float *ms_tota
     }
     cudaStream_t s = c->stream;
     if (flush_l2 && !c->flush_buf) {
-        c->flush_bytes = (size_t)256 << 20;  // 2x the 126 MB L2
+        c->flush_bytes = (size_t)128 << 20;  // more than 2x the 50 MB L2 of an H100
         SB_TRY(dev_alloc(&c->flush_buf, c->flush_bytes, s));
     }
     float total = 0.f;

@@ -61,8 +61,8 @@ static int init_locked(int ordinal)
     SB_CUDA(cudaSetDevice(ordinal));
     SB_CUDA(cudaGetDeviceProperties(&g_prop, ordinal));
 #ifndef SB_EMU
-    if (g_prop.major != 10) {
-        set_error("device %d (%s) is sm_%d%d; libstitch_b200 is built for sm_100a only and has no fallback", ordinal, g_prop.name,
+    if (g_prop.major != 9 || g_prop.minor != 0) {
+        set_error("device %d (%s) is sm_%d%d; libstitch_b200 is built for sm_90a only and has no fallback", ordinal, g_prop.name,
                   g_prop.major, g_prop.minor);
         return SB_ERR_NO_DEVICE;
     }
@@ -112,7 +112,7 @@ void dev_free(void *p, cudaStream_t s)
 extern "C" {
 
 const char *sb_last_error(void) { return sb::g_err; }
-const char *sb_version(void) { return "stitch_b200 0.1 (sm_100a)"; }
+const char *sb_version(void) { return "stitch_b200 0.1 (sm_90a)"; }
 
 int sb_init(int device_ordinal)
 {

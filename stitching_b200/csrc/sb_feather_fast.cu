@@ -12,8 +12,8 @@
 //            up d(y) = -y + min_{j>=y}(r(j) + j).  A column is cut into SB_DT_CHUNKS row chunks with one thread each:
 //            k_dt_cols_summary reduces every chunk to its two minima, k_dt_cols_apply combines the minima of the chunks
 //            above / below into carries and walks its own chunk down and up -- the serial chain is h / 32 rows instead
-//            of 2 h (the one-thread-per-column sweeps of k_dt_cols_batched took 1.1 of the 1.5 ms of a 16 x 2000x1500
-//            feather blend).  All images of the blend in one launch each.
+//            of 2 h (the one-thread-per-column sweeps of k_dt_cols_batched were most of a 16 x 2000x1500 feather
+//            blend where they were measured).  All images of the blend in one launch each.
 // "No zero anywhere" stays at DT_INF and becomes weight 1, as with OpenCV (the image border is not a zero).
 #include <cstdlib>
 

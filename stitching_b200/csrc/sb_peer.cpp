@@ -1,19 +1,17 @@
 // sb_peer.cpp -- the slab exchange of the sharded composite as direct NVLink stores (no reference counterpart: the
 // reference is single-process; this is SURVEY.md 8(e)).
 //
-// Round 1 moved the slabs with grouped ncclSend / ncclRecv on a communication stream: at 8 GPUs the exchange ran at
-// ~127 GB/s per rank and the collapse waited for it (VERDICT r1, item 8).  Here every rank keeps the slabs it RECEIVES
+// Round 1 moved the slabs with grouped ncclSend / ncclRecv on a communication stream: at 8 GPUs the exchange ran far
+// below link rate and the collapse waited for it (VERDICT r1, item 8).  Here every rank keeps the slabs it RECEIVES
 // in one cudaMalloc'ed arena, exports it with CUDA IPC, and maps its neighbours' arenas.  The partial-sum launches
 // (k_collapse_fast with `partial` set) write their slabs into local send buffers and the copy engines move them into
 // the owners' arenas (cudaMemcpyAsync on the mapped peer pointers: NVLink DMA at link rate, no SM, no NCCL kernel, on
 // a second stream beside the pyramid kernels).  Storing the slabs from the kernels straight into the peers' arenas is
-// available too (SB_PEER=direct) -- measured on 2 B200s it LOSES: the 2- and 4-byte scattered stores of that kernel
-// cross NVLink as small partial writes, partial_l0 0.025 -> 0.179 ms, step 0.97 -> 1.21 ms
-// (profiles/bench_r02_e_2gpu_direct_stores.json).  The ranks order themselves with four flags per pair, written by
+// available too (SB_PEER=direct) -- it lost where it was measured: the 2- and 4-byte scattered stores of that kernel
+// cross NVLink as small partial writes.  The ranks order themselves with four flags per pair, written by
 // stream memory operations (cuStreamWriteValue32: stream-ordered behind the copy, no host round trip) and awaited by a
 // one-warp polling kernel (k_wait_flags, sb_util.cu) right before the kernel that reads the slab -- cuStreamWaitValue32
-// was measured too and lost: enqueued ahead, the front end evaluates those waits in batches and a step went from
-// 0.92 to 1.86 ms (profiles/bench_r02_e_2gpu_streamwait.json):
+// was measured too and lost: enqueued ahead, the front end evaluates those waits in batches:
 //   data[part][p]  in the RECEIVER's arena: rank p has finished writing part `part` (0: level 0, 1: the coarser
 //                  levels) of step `value`;
 //   consumed[p]    in the SENDER's arena: rank p has read the slabs of step `value` (the next step may overwrite them).

@@ -247,8 +247,8 @@ int BlendPlan::allocate(cudaStream_t s)
     col_dev = (ColDesc *)(base + col_off);
     pyr_dev = (PyrDesc *)(base + pyr_off);
     tail_state_dev = (unsigned *)(base + tail_off);
-    // fused tail (sb_tail.cu): OFF by default -- measured on B200 (profiles/bench_r02_c_tail.json) the one-launch
-    // per-pixel version of levels 3..7 takes 0.19 ms against 0.11 ms for the twelve tuned per-level launches.
+    // fused tail (sb_tail.cu): OFF by default -- where it was measured, the one-launch per-pixel version of levels
+    // 3..7 was slower than the twelve tuned per-level launches.
     // SB_TAIL_FROM=<level> enables it from that level on (A/B measurements, tests).
     tail_from = 1 << 30;
     if (kind == SB_BLEND_MULTIBAND && active_count < 0 && n > 0) {

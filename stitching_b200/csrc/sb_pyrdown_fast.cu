@@ -25,7 +25,7 @@
 // integer and its value does not depend on the summation order: the level-1 weight is V / 256 with V = the integer
 // 5x5 filter of the mask BITS.  The mask byte already rides through both integer passes in the spare 16-bit lane next
 // to green (V_m = 255 V <= 65280), so the float path -- half of the kernel's instructions in the profile of the generic
-// version (profiles/ncu_r02_i_*) -- disappears: V = (257 V_m + 65535) >> 16, one conversion, one exact multiply.
+// version -- disappears: V = (257 V_m + 65535) >> 16, one conversion, one exact multiply.
 // The levels built from such weights stay exact for two more steps: level-1 weights are V / 2^8 (V <= 2^8), level-2
 // weights V / 2^16, and every partial sum of the next pyrDown is an integer multiple of that unit not above 2^24 -- inside
 // the float's 24-bit significand -- so for l = 1, 2 BIN means "any summation order": the kernel evaluates one instead of

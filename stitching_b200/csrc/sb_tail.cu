@@ -1,8 +1,8 @@
 // sb_tail.cu -- the tail of the multiband pyramid in ONE launch: pyrDown of levels T .. nb-1 of every fed image, then
 // accumulate + normalise + collapse of levels nb .. T of the panorama.
 //
-// From level 3 on a level is a few hundred thousand pixels: the round-1 launch list shows twelve launches of 9-12 us
-// each for them (pyrDown l3-l6, collapse l7-l3, ~0.11 ms of a 1.39 ms step) at under 10 % occupancy -- launch latency
+// From level 3 on a level is a few hundred thousand pixels: the round-1 launch list shows twelve short launches
+// each for them (pyrDown l3-l6, collapse l7-l3) at under 10 % occupancy -- launch latency
 // and the serial row walk of the tuned kernels, not work.  Here a persistent grid (two CTAs per SM) runs the phases
 // back to back with a grid barrier in between, every phase as independent per-pixel gathers (sb_gather.cuh, the same
 // functions as the simple kernels: bit-identical arithmetic, either level layout).  No location is read before the

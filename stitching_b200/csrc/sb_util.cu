@@ -53,15 +53,15 @@ __global__ void k_selftest_division(unsigned long long n, unsigned long long see
 
 int launch_selftest_division(unsigned long long n, unsigned long long seed, int mode, unsigned long long *bad_dev, cudaStream_t s)
 {
-    launch(k_selftest_division, dim3(148 * 8), dim3(256), 0, s, n, seed, mode, bad_dev);
+    launch(k_selftest_division, dim3(sm_count() * 8), dim3(256), 0, s, n, seed, mode, bad_dev);
     return launch_check("k_selftest_division");
 }
 
 #ifndef SB_EMU
 // One warp polls up to 32 flags in this device's memory until each has reached `value` (flags only ever grow).  The
 // sharded composite orders its ranks with this instead of cuStreamWaitValue32: an unsatisfied stream wait sends the
-// channel back to the runlist and is re-examined a timeslice later -- measured on 2 B200s that turned a 0.92 ms step
-// into 1.86 ms once steps were enqueued ahead (profiles/bench_r02_e_2gpu_streamwait.json); a polling warp sees the
+// channel back to the runlist and is re-examined a timeslice later, which slows the step down badly once steps are
+// enqueued ahead; a polling warp sees the
 // peer's write within a microsecond.
 __global__ void k_wait_flags(const volatile unsigned *flags, unsigned mask, unsigned value)
 {
@@ -126,7 +126,7 @@ int launch_timelapse_frame(const uint8_t *src8, const int16_t *src16, long long 
 int launch_flush_l2(void *buf, size_t bytes, cudaStream_t s)
 {
     static unsigned v = 0;
-    launch(k_flush, dim3(148 * 8), dim3(256), 0, s, (uint4 *)buf, bytes / sizeof(uint4), ++v);
+    launch(k_flush, dim3(sm_count() * 8), dim3(256), 0, s, (uint4 *)buf, bytes / sizeof(uint4), ++v);
     return launch_check("k_flush");
 }
 }  // namespace sb

@@ -19,11 +19,12 @@ class _Handle:
 
     def __init__(self, ptr):
         self.ptr = ptr
+        self.L = _lib.lib()  # released by the library that made it, whichever is bound later
 
     def __del__(self):
         try:
             if self.ptr:
-                _lib.lib().sb_devimg_release(self.ptr)
+                self.L.sb_devimg_release(self.ptr)
                 self.ptr = None
         except Exception:  # interpreter shutdown
             pass

@@ -1,4 +1,4 @@
-"""B200 drop-in for the FINAL-resolution half of stitching.exposure_error_compensator.ExposureErrorCompensator
+"""GPU drop-in for the FINAL-resolution half of stitching.exposure_error_compensator.ExposureErrorCompensator
 (reference: stitching/exposure_error_compensator.py).
 
 Gain estimation (`feed`, at LOW resolution, stitcher.py:211) stays with OpenCV's compensators.  `apply` -- run on every

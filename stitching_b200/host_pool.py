@@ -2,7 +2,7 @@
 
 The reference's calls return fresh ndarrays (warper.py:43-68, blender.py:43-48).  A fresh `np.empty` of tens of
 megabytes is untouched virtual memory: the device-to-host copy into it first faults every page in and then goes through
-the driver's staging buffer -- on the B200 boxes that was most of a drop-in stitch (bench.py `e2e.dropin.stage_ms`).
+the driver's staging buffer -- where it was measured that was most of a drop-in stitch (bench.py `e2e.dropin.stage_ms`).
 Here the arrays live in buffers from `sb_host_alloc` (cudaHostAlloc): the copy is one DMA at PCIe speed, and a buffer
 whose last ndarray view died goes back to a free list, so the next stitch of the same rig allocates nothing.
 
@@ -20,7 +20,7 @@ from . import _lib
 
 _GRAIN = 1 << 20  # buffers come in multiples of 1 MiB so that rigs with slightly different rois share them
 _lock = threading.Lock()
-_free = {}        # rounded size -> [address, ...]
+_free = {}        # rounded size -> [(address, library that allocated it), ...]
 _total = 0        # bytes of page-locked memory alive (handed out + cached)
 
 
@@ -31,9 +31,9 @@ def _limit():
         return 8192 << 20
 
 
-def _release(addr, size):
+def _release(block, size):
     with _lock:
-        _free.setdefault(size, []).append(addr)
+        _free.setdefault(size, []).append(block)
 
 
 def empty(shape, dtype=np.uint8):
@@ -45,11 +45,11 @@ def empty(shape, dtype=np.uint8):
     if nbytes < (1 << 18):
         return np.empty(shape, dtype)
     size = (nbytes + _GRAIN - 1) // _GRAIN * _GRAIN
-    addr, drop = None, []
+    block, drop = None, []
     with _lock:
         lst = _free.get(size)
         if lst:
-            addr = lst.pop()
+            block = lst.pop()
         else:
             # make room from the cache of other sizes before giving up on page-locked memory
             for s, cached in list(_free.items()):
@@ -58,19 +58,20 @@ def empty(shape, dtype=np.uint8):
                     _total -= s
             if _total + size <= _limit():
                 _total += size
-                addr = 0
-    for a in drop:
-        _lib.lib().sb_host_free(a)
-    if addr is None:
+                block = (0, None)
+    for a, L in drop:
+        L.sb_host_free(a)
+    if block is None:
         return np.empty(shape, dtype)
-    if addr == 0:
-        addr = _lib.lib().sb_host_alloc(size)
-        if not addr:
+    if block[0] == 0:
+        L = _lib.lib()  # a buffer goes back to the library that allocated it, whichever library is bound later
+        block = (L.sb_host_alloc(size), L)
+        if not block[0]:
             with _lock:
                 _total -= size
             return np.empty(shape, dtype)
-    buf = (C.c_uint8 * size).from_address(addr)
-    fin = weakref.finalize(buf, _release, addr, size)
+    buf = (C.c_uint8 * size).from_address(block[0])
+    fin = weakref.finalize(buf, _release, block, size)
     fin.atexit = False  # at interpreter exit the process's memory goes away as a whole
     return np.frombuffer(buf, dtype=dtype, count=nbytes // dtype.itemsize).reshape(shape)
 
@@ -79,8 +80,8 @@ def trim():
     """Gives the cached buffers back to the driver (the handed-out ones follow when their arrays die)."""
     global _total
     with _lock:
-        items = [(a, s) for s, lst in _free.items() for a in lst]
+        items = [(b, s) for s, lst in _free.items() for b in lst]
         _free.clear()
         _total -= sum(s for _, s in items)
-    for a, _ in items:
-        _lib.lib().sb_host_free(a)
+    for (a, L), _ in items:
+        L.sb_host_free(a)

@@ -1,4 +1,4 @@
-"""B200 drop-in for the resampling step of stitching.images.Images (reference: stitching/images.py:120-123).
+"""GPU drop-in for the resampling step of stitching.images.Images (reference: stitching/images.py:120-123).
 
 `Images.resize_img_by_scaler(scaler, size, img)` produces the MEDIUM / LOW / FINAL resolution inputs of the pipeline
 with `cv.resize(img, desired_size, interpolation=cv.INTER_LINEAR_EXACT)`; here the same bit-exact fixed-point bilinear

@@ -1,4 +1,4 @@
-"""B200 drop-in for the FINAL-resolution half of stitching.seam_finder.SeamFinder (reference: stitching/seam_finder.py).
+"""GPU drop-in for the FINAL-resolution half of stitching.seam_finder.SeamFinder (reference: stitching/seam_finder.py).
 
 Seam estimation itself (`SeamFinder.find`, OpenCV's graph-cut / dynamic-programming finders at LOW resolution) stays
 with the reference.  `resize` -- the step that produces the blend mask of every image at FINAL resolution

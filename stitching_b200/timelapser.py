@@ -1,4 +1,4 @@
-"""B200 drop-in for stitching.timelapser.Timelapser (reference: stitching/timelapser.py:7-56).
+"""GPU drop-in for stitching.timelapser.Timelapser (reference: stitching/timelapser.py:7-56).
 
 The timelapser is the other consumer of the warped FINAL-resolution frames (stitcher.py:242-252): every frame is the
 canvas of the prepared roi with ONE warped image pasted at its corner.  Same class constants, constructor, method names

@@ -1,7 +1,7 @@
-"""B200 drop-in for stitching.warper.Warper (reference: stitching/warper.py:7-94).
+"""GPU drop-in for stitching.warper.Warper (reference: stitching/warper.py:7-94).
 
 Same class constants, method names, argument meaning and return types; the OpenCV calls behind them
-(cv.PyRotationWarper.warp / warpRoi) are replaced by libstitch_b200's fused sm_100a warp kernel.  All sixteen
+(cv.PyRotationWarper.warp / warpRoi) are replaced by libstitch_b200's fused sm_90a warp kernel.  All sixteen
 projections of WARP_TYPE_CHOICES are served bit-identically: spherical, cylindrical, plane, affine and mercator
 project on the device from separable trig tables; the other eleven (fisheye, stereographic, compressedPlane*,
 panini*, transverseMercator) are not separable and must match glibc's sinf / atan2f / tanf ... bit for bit, so
@@ -102,7 +102,7 @@ class Warper:
         if img is not None:
             img = np.asarray(img)
             if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
-                raise _lib_argument_error("the B200 warp path takes uint8 HxWx3 images")
+                raise _lib_argument_error("the GPU warp path takes uint8 HxWx3 images")
             if img.strides[2] != 1 or img.strides[1] != 3 or img.strides[0] < img.shape[1] * 3:
                 img = np.ascontiguousarray(img)  # e.g. a column-sliced crop keeps row pitch; anything odder is copied
             size = (img.shape[1], img.shape[0])

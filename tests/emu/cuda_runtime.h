@@ -64,7 +64,7 @@ static inline const char *cudaGetErrorString(cudaError_t) { return "emu"; }
 static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceCount(int *n) { *n = 8; return cudaSuccess; }
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
-static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { std::memset(p, 0, sizeof *p); std::strcpy(p->name, "EMU (tests only)"); p->major = 10; p->multiProcessorCount = 148; return cudaSuccess; }
+static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { std::memset(p, 0, sizeof *p); std::strcpy(p->name, "EMU (tests only)"); p->major = 9; p->multiProcessorCount = 132; return cudaSuccess; }
 static inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, unsigned) { *s = (cudaStream_t)std::malloc(1); return cudaSuccess; }
 static inline cudaError_t cudaStreamDestroy(cudaStream_t s) { std::free(s); return cudaSuccess; }
 static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }

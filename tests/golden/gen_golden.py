@@ -1,14 +1,17 @@
 """Generate the committed golden vectors from the UNMODIFIED reference.
 
-Runs only in the build container, where /root/reference (OpenStitching/stitching v0.7.0) and its numeric
-backend cv2 4.13.0 are importable:
+Needs a checkout of the reference (OpenStitching/stitching v0.7.0) and its numeric backend cv2 4.13.0:
 
-    python tests/golden/gen_golden.py
+    python tests/golden/gen_golden.py <path of the reference checkout> [generator ...]
+
+(all generators by default; e.g. `reference` rewrites golden_reference.npz only).
 
 Every expected output below is produced by the reference's own classes
 (stitching.warper.Warper, stitching.blender.Blender -- reference files stitching/warper.py, stitching/blender.py)
 or, for the pyramid primitives, by the cv2 calls OpenCV's blender makes internally.  The fixtures are replayed by
 tests/test_oracle_golden.py (CPU oracle) and tests/test_gpu_parity.py (CUDA path); neither needs the reference.
+gen_reference pins the seeded cases of tests/reference_cases.py for tests/test_vs_reference_live.py and
+tests/test_dropin_pipeline.py.
 """
 import hashlib
 import os
@@ -18,13 +21,16 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.join(HERE, ".."))
+if __name__ == "__main__":
+    sys.path.insert(0, os.path.abspath(sys.argv[1]))
 
 import cv2 as cv  # noqa: E402
 from stitching.blender import Blender as RefBlender  # noqa: E402
 from stitching.warper import Warper as RefWarper  # noqa: E402
 
 from stitching_b200 import rigs  # noqa: E402
+import replay  # noqa: E402
 
 
 def rot(rx, ry, rz):
@@ -81,7 +87,7 @@ def gen_warp():
         out[f"roi_{i}"] = np.array(wr.warp_roi((W, H), cam, aspect), np.int64)
         out[f"img_{i}"] = wr.warp_image(img, cam, aspect)
         out[f"mask_{i}"] = wr.create_and_warp_mask((W, H), cam, aspect)
-    np.savez_compressed(os.path.join(HERE, "golden_warp.npz"), **out)
+    replay.save("golden_warp.npz", out)
     print("warp cases", len(cases))
 
 
@@ -143,7 +149,7 @@ def gen_blend():
             out[f"corner_{i}_{j}"] = np.array(corners[j], np.int64)
         out[f"pano_{i}"] = pano
         out[f"pmask_{i}"] = pmask
-    np.savez_compressed(os.path.join(HERE, "golden_blend.npz"), **out)
+    replay.save("golden_blend.npz", out)
     print("blend cases", len(specs))
 
 
@@ -166,7 +172,7 @@ def gen_pyr():
     m = (rng.random((40, 60)) > 0.2).astype(np.uint8) * 255
     out["dt_mask"] = m
     out["dt_l1"] = cv.distanceTransform(m, cv.DIST_L1, 3)
-    np.savez_compressed(os.path.join(HERE, "golden_pyr.npz"), **out)
+    replay.save("golden_pyr.npz", out)
     print("pyr cases", len(shapes))
 
 
@@ -199,7 +205,7 @@ def gen_e2e():
         out[f"{name}_pano"] = pano
         out[f"{name}_pmask"] = pmask
         print(name, "pano", pano.shape)
-    np.savez_compressed(os.path.join(HERE, "golden_e2e.npz"), **out)
+    replay.save("golden_e2e.npz", out)
 
 
 def gen_seam():
@@ -235,7 +241,7 @@ def gen_seam():
         out[f"mask_{i}"] = m
         out[f"out_{i}"] = got.get() if hasattr(got, "get") else np.asarray(got)
     out["n"] = len(cases)
-    np.savez_compressed(os.path.join(HERE, "golden_seam.npz"), **out)
+    replay.save("golden_seam.npz", out)
     print("seam cases", len(cases))
 
 
@@ -269,7 +275,7 @@ def gen_gain():
             out[f"out_{k}"] = got.get() if hasattr(got, "get") else np.asarray(got)
             k += 1
     out["n"] = k
-    np.savez_compressed(os.path.join(HERE, "golden_gain.npz"), **out)
+    replay.save("golden_gain.npz", out)
     print("gain cases", k)
 
 
@@ -291,7 +297,7 @@ def gen_resize():
         out[f"out_{k}"] = RefImages.resize_img_by_scaler(scaler, (w, h), img)
         k += 1
     out["n"] = k
-    np.savez_compressed(os.path.join(HERE, "golden_resize.npz"), **out)
+    replay.save("golden_resize.npz", out)
     print("resize cases", k, [tuple(out[f"size_{i}"]) for i in range(k)])
 
 
@@ -323,20 +329,249 @@ def gen_timelapse():
                 out[f"frame_{k}_{i}"] = t.get_frame()
             k += 1
     out["n"] = k
-    np.savez_compressed(os.path.join(HERE, "golden_timelapse.npz"), **out)
+    replay.save("golden_timelapse.npz", out)
     print("timelapse cases", k, [out[f"frame_{i}_0"].shape for i in range(k)])
+
+
+def gen_reference():
+    """The seeded cases of tests/reference_cases.py through the reference's classes, and one run of its Stitcher on
+    synthetic views with every call across the hot-path boundary recorded (Warper, Images.resize_img_by_scaler,
+    ExposureErrorCompensator.apply, SeamFinder.resize, Blender): what the calls got that cannot be rebuilt from the seeds
+    (cameras, gains, LOW-resolution seam masks), and digests of everything else."""
+    import reference_cases as rc
+    from stitching.exposure_error_compensator import ExposureErrorCompensator as RefCompensator
+    from stitching.images import Images as RefImages
+    from stitching.seam_finder import SeamFinder as RefSeamFinder
+    from stitching.timelapser import Timelapser as RefTimelapser
+
+    assert tuple(RefWarper.WARP_TYPE_CHOICES) == rc.WARP_TYPES and tuple(RefCompensator.COMPENSATOR_CHOICES) == rc.COMPENSATORS
+    pins = rc.Pins(record=True)
+    for key, wtype, cam, scale, aspect, img in rc.warp_cases():
+        wr = RefWarper(wtype)
+        wr.scale = scale
+        size = (img.shape[1], img.shape[0])
+        roi = pins.value(key + ".roi", tuple(int(v) for v in wr.warp_roi(size, cam, aspect)))
+        if roi[2] * roi[3] > 4_000_000:
+            continue  # a degenerate draw (horizon in view): the tests check the rect only
+        pins.array(key + ".img", wr.warp_image(img, cam, aspect))
+        pins.array(key + ".mask", wr.create_and_warp_mask(size, cam, aspect))
+    for trial, kind, strength, corners, sizes, imgs, masks in rc.blend_cases():
+        b = RefBlender(kind, strength)
+        b.prepare(corners, sizes)
+        for img, m, c in zip(imgs, masks, corners):
+            b.feed(img, m, c)
+        pano, pmask = b.blend()
+        pins.array(f"blend.{trial}.pano", pano)
+        pins.array(f"blend.{trial}.mask", pmask)
+        for tl_kind in ("as_is", "crop"):
+            t = RefTimelapser(tl_kind)
+            t.initialize(corners, sizes)
+            for i, (img, c) in enumerate(zip(imgs, corners)):
+                t.process_frame(img, c)
+                try:
+                    pins.array(f"timelapse.{trial}.{tl_kind}.{i}", t.get_frame())
+                except cv.error:  # rects that touch in a line: get_frame fails on the empty canvas
+                    pins.value(f"timelapse.{trial}.{tl_kind}.{i}", "raises cv2.error")
+    for case in rc.final_resolution_cases():
+        if case[0] == "seam":
+            _, t, seam, mask = case
+            pins.array(f"seam.{t}", RefSeamFinder.resize(cv.UMat(seam), mask))
+        elif case[0] == "resize":
+            _, t, img, size = case
+            pins.array(f"resize.{t}", RefImages.resize_img_by_scaler(rc.Scaler(size), (img.shape[1], img.shape[0]), img))
+        else:
+            _, kind, corners, imgs, masks = case
+            comp = RefCompensator(kind, 1, 16)
+            comp.feed(corners, imgs, masks)
+            for i in range(len(imgs)):
+                if kind != "no":
+                    pins.value(f"gain.{kind}.{i}.gains", np.asarray(comp.compensator.getMatGains()[i]))
+                pins.array(f"gain.{kind}.{i}", comp.apply(i, corners[i], imgs[i].copy(), masks[i]))
+    for trial, wtype, btype, cams, imgs in rc.dropin_cases():
+        key = f"dropin.{trial}"
+        w = RefWarper(wtype)
+        w.set_scale(cams)
+        sizes = [(img.shape[1], img.shape[0]) for img in imgs]
+        warped = list(w.warp_images(imgs, cams))
+        masks = list(w.create_and_warp_masks(sizes, cams))
+        corners, wsizes = w.warp_rois(sizes, cams)
+        b = RefBlender(btype, 5)
+        b.prepare(corners, wsizes)
+        for img, m, c in zip(warped, masks, corners):
+            b.feed(img, m, c)
+        pano, pmask = b.blend()
+        t = RefTimelapser("as_is")
+        t.initialize(corners, wsizes)
+        t.process_frame(warped[1], corners[1])
+        pins.value(key + ".corners", np.array(corners, np.int64))
+        pins.value(key + ".sizes", np.array(wsizes, np.int64))
+        for i in range(len(imgs)):
+            pins.array(f"{key}.warped.{i}", warped[i])
+            pins.array(f"{key}.mask.{i}", masks[i])
+        pins.array(key + ".pano", pano)
+        pins.array(key + ".pmask", pmask)
+        pins.array(key + ".frame", t.get_frame())
+    record_pipelines(pins, rc)
+    pins.save()
+    print("reference pins", len(pins.data), os.path.getsize(rc.PATH) // 1024, "KiB")
+
+
+def record_pipeline(pins, rc, name, run, sources):
+    """run(stitching) drives the reference's pipeline on `sources`; every call across the hot-path boundary -- at the
+    bindings stitching_b200.install() replaces -- is recorded as pipe.<name>.<k>.*  An input that is neither a source nor
+    what an earlier recorded call returned (the colour seam masks seam_finder.blend_seam_masks feeds) is stored as it is."""
+    import importlib
+
+    import stitching
+    from stitching.exposure_error_compensator import ExposureErrorCompensator as RefCompensator
+    from stitching.images import Images as RefImages
+    from stitching.seam_finder import SeamFinder as RefSeamFinder
+    from stitching.timelapser import Timelapser as RefTimelapser
+
+    log = []
+
+    class RecWarper(RefWarper):
+        def warp_image(self, img, camera, aspect=1):
+            out = super().warp_image(img, camera, aspect)
+            log.append(dict(kind="warp_image", type=self.warper_type, scale=self.scale, camera=rc.camera_value(camera), aspect=aspect,
+                            input=rc.digest(img), out=rc.digest(out)))
+            return out
+
+        def create_and_warp_mask(self, size, camera, aspect=1):
+            out = super().create_and_warp_mask(size, camera, aspect)
+            log.append(dict(kind="warp_mask", type=self.warper_type, scale=self.scale, camera=rc.camera_value(camera), aspect=aspect,
+                            size=np.array(size, np.int64), out=rc.digest(out)))
+            return out
+
+        def warp_roi(self, size, camera, aspect=1):
+            out = super().warp_roi(size, camera, aspect)
+            log.append(dict(kind="warp_roi", type=self.warper_type, scale=self.scale, camera=rc.camera_value(camera), aspect=aspect,
+                            size=np.array(size, np.int64), roi=np.array(out, np.int64)))
+            return out
+
+    class RecBlender(RefBlender):
+        def prepare(self, corners, sizes):
+            log.append(dict(kind="prepare", type=self.blender_type, strength=self.blend_strength, corners=np.array(corners, np.int64),
+                            sizes=np.array(sizes, np.int64)))
+            super().prepare(corners, sizes)
+
+        def feed(self, img, mask, corner):
+            log.append(dict(kind="feed", input=rc.digest(img), mask=rc.digest(mask), mask_type=type(mask).__name__, corner=np.array(corner, np.int64),
+                            arrays={"input": np.array(img.get() if hasattr(img, "get") else img), "mask": np.array(mask.get() if hasattr(mask, "get") else mask)}))
+            super().feed(img, mask, corner)
+
+        def blend(self):
+            pano, mask = super().blend()
+            log.append(dict(kind="blend", pano=rc.digest(pano), mask=rc.digest(mask)))
+            return pano, mask
+
+    class RecTimelapser(RefTimelapser):
+        def __init__(self, timelapse=RefTimelapser.DEFAULT_TIMELAPSE, timelapse_prefix=RefTimelapser.DEFAULT_TIMELAPSE_PREFIX):
+            super().__init__(timelapse, timelapse_prefix)
+            self.rec_type = timelapse
+
+        def initialize(self, corners, sizes):
+            log.append(dict(kind="tl_init", type=self.rec_type, corners=np.array(corners, np.int64), sizes=np.array(sizes, np.int64)))
+            super().initialize(corners, sizes)
+
+        def process_frame(self, img, corner):
+            super().process_frame(img, corner)
+            log.append(dict(kind="tl_frame", input=rc.digest(img), corner=np.array(corner, np.int64), out=rc.digest(self.get_frame())))
+
+    ref_resize, ref_apply, ref_img_resize = RefSeamFinder.resize, RefCompensator.apply, RefImages.resize_img_by_scaler
+
+    def rec_resize(seam_mask, mask):
+        out = ref_resize(seam_mask, mask)
+        log.append(dict(kind="seam_resize", seam=np.array(seam_mask.get() if hasattr(seam_mask, "get") else seam_mask), seam_type=type(seam_mask).__name__,
+                        mask=rc.digest(mask), out=rc.digest(out), out_type=type(out).__name__))
+        return out
+
+    def rec_apply(self, *args):
+        idx, _corner, img, _mask = args
+        before = rc.digest(img)
+        gains = self.compensator.getMatGains()  # none for the "no" compensator
+        out = ref_apply(self, *args)
+        e = dict(kind="gain_apply", input=before, out=rc.digest(out))
+        if idx < len(gains):
+            e["gain"] = np.array(gains[idx]).copy()
+        log.append(e)
+        return out
+
+    def rec_img_resize(scaler, size, img):
+        out = ref_img_resize(scaler, size, img)
+        log.append(dict(kind="img_resize", input=rc.digest(img), size=np.array(scaler.get_scaled_img_size(size), np.int64), out=rc.digest(out)))
+        return out
+
+    rec = {"Warper": RecWarper, "Blender": RecBlender, "Timelapser": RecTimelapser}
+    saved = []
+    for mod, names in (("stitcher", ("Warper", "Blender", "Timelapser")), ("cropper", ("Blender",)), ("seam_finder", ("Blender",)),
+                       ("verbose", ("Warper", "Blender", "Timelapser"))):
+        m = importlib.import_module(f"stitching.{mod}")
+        for n in names:
+            if hasattr(m, n):
+                saved.append((m, n, getattr(m, n)))
+                setattr(m, n, rec[n])
+    RefSeamFinder.resize = staticmethod(rec_resize)
+    RefCompensator.apply = rec_apply
+    RefImages.resize_img_by_scaler = staticmethod(rec_img_resize)
+    try:
+        run(stitching)
+    finally:
+        RefSeamFinder.resize = staticmethod(ref_resize)
+        RefCompensator.apply = ref_apply
+        RefImages.resize_img_by_scaler = staticmethod(ref_img_resize)
+        for m, n, v in saved:
+            setattr(m, n, v)
+    known = {rc.digest(v) for v in sources}
+    for e in log:
+        for field, v in e.pop("arrays", {}).items():
+            if e[field] not in known:
+                e[field + "_value"] = v
+        if "out" in e:
+            known.add(e["out"])
+    pins.value(f"pipe.{name}.n", len(log))
+    for k, e in enumerate(log):
+        for field, v in e.items():
+            pins.value(f"pipe.{name}.{k}.{field}", v)
+    print("pipeline", name, len(log), "calls")
+
+
+def record_pipelines(pins, rc):
+    """The reference's Stitcher, stitch_verbose, two other warper types, a timelapse run, one Stitcher for two image sets
+    and AffineStitcher, each on synthetic inputs (tests/reference_cases.py)."""
+    import tempfile
+
+    S = rc.PIPELINE_SETTINGS
+    views = rc.synthetic_views(cv)
+    record_pipeline(pins, rc, "stitch", lambda st: st.Stitcher(**S).stitch([v.copy() for v in views]), views)
+    with tempfile.TemporaryDirectory() as d:
+        record_pipeline(pins, rc, "verbose", lambda st: st.Stitcher(**S).stitch_verbose([v.copy() for v in views], verbose_dir=d), views)
+    for wtype in ("fisheye", "compressedPlaneA2B1"):
+        record_pipeline(pins, rc, wtype, lambda st: st.Stitcher(warper_type=wtype, **S).stitch([v.copy() for v in views]), views)
+    with tempfile.TemporaryDirectory() as d:
+        names = []
+        for i, v in enumerate(views):
+            names.append(os.path.join(d, f"view{i}.png"))
+            cv.imwrite(names[-1], v)
+        record_pipeline(pins, rc, "timelapse", lambda st: st.Stitcher(timelapse="as_is", **S).stitch(names), views)
+
+    def two_sets(st):
+        s = st.Stitcher(**S)
+        s.stitch([v.copy() for v in views])
+        s.stitch([v.copy() for v in views[:2]])
+        s.stitch([v.copy() for v in views])
+
+    record_pipeline(pins, rc, "two_sets", two_sets, views)
+    scans = rc.synthetic_scans(cv)
+    record_pipeline(pins, rc, "affine", lambda st: st.AffineStitcher(**S).stitch([s.copy() for s in scans]), scans)
 
 
 if __name__ == "__main__":
     print("cv2", cv.__version__)
-    gen_warp()
-    gen_blend()
-    gen_pyr()
-    gen_e2e()
-    gen_seam()
-    gen_gain()
-    gen_resize()
-    gen_timelapse()
+    gens = {"warp": gen_warp, "blend": gen_blend, "pyr": gen_pyr, "e2e": gen_e2e, "seam": gen_seam, "gain": gen_gain,
+            "resize": gen_resize, "timelapse": gen_timelapse, "reference": gen_reference}
+    for name in sys.argv[2:] or gens:
+        gens[name]()
     for f in sorted(os.listdir(HERE)):
         if f.endswith(".npz"):
             print(f, os.path.getsize(os.path.join(HERE, f)) // 1024, "KiB")

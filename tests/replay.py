@@ -11,8 +11,48 @@ import numpy as np
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
+PART_BYTES = 900_000  # an archive above this is written as parts <name>_part<k>.npz, each under 1 MB
+
+
 def load(name):
-    return np.load(os.path.join(GOLDEN, name), allow_pickle=False)
+    """The arrays of golden archive `name`, or of its parts when it was written in parts (save)."""
+    path = os.path.join(GOLDEN, name)
+    if os.path.exists(path):
+        return np.load(path, allow_pickle=False)
+    stem = name[:-len(".npz")]
+    parts, k = {}, 0
+    while os.path.exists(os.path.join(GOLDEN, f"{stem}_part{k}.npz")):
+        with np.load(os.path.join(GOLDEN, f"{stem}_part{k}.npz"), allow_pickle=False) as z:
+            parts.update({key: z[key] for key in z.files})
+        k += 1
+    assert parts, f"{name}: no such golden archive"
+    return parts
+
+
+def save(name, arrays):
+    """Write golden archive `name` (compressed), in parts of at most about PART_BYTES when it is larger, keys in order."""
+    import io
+    import zlib
+
+    def packed(a):
+        buf = io.BytesIO()
+        np.save(buf, np.asarray(a), allow_pickle=False)
+        return len(zlib.compress(buf.getvalue()))
+
+    groups, size = [[]], 0
+    for key, a in arrays.items():
+        n = packed(a)
+        if groups[-1] and size + n > PART_BYTES:
+            groups.append([])
+            size = 0
+        groups[-1].append(key)
+        size += n
+    stem = os.path.join(GOLDEN, name[:-len(".npz")])
+    if len(groups) == 1:
+        np.savez_compressed(stem + ".npz", **arrays)
+        return
+    for k, keys in enumerate(groups):
+        np.savez_compressed(f"{stem}_part{k}.npz", **{key: arrays[key] for key in keys})
 
 
 def diff_report(got, exp, what):

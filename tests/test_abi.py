@@ -37,7 +37,7 @@ def test_binding_covers_the_header():
     _lib.bind(_lib.LIB_PATH)  # attaches every prototype
 
 
-def test_library_targets_sm100a_only():
+def test_library_targets_sm90a_only():
     import shutil
     import subprocess
 
@@ -46,7 +46,7 @@ def test_library_targets_sm100a_only():
         pytest.skip("cuobjdump not available")
     out = subprocess.run([cuobjdump, "--list-elf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_no_cpu_fallback_without_a_gpu():

@@ -36,7 +36,7 @@ def test_native_library_is_the_one_running(cuda_lib):
     name = C.create_string_buffer(128)
     sm, maj, mnr = C.c_int(), C.c_int(), C.c_int()
     assert cuda_lib.sb_device_info(name, 128, C.byref(sm), C.byref(maj), C.byref(mnr)) == 0
-    assert maj.value == 10, f"not an sm_100 device: {name.value} sm_{maj.value}{mnr.value}"
+    assert (maj.value, mnr.value) == (9, 0), f"not an sm_90 device: {name.value} sm_{maj.value}{mnr.value}"
     before = cuda_lib.sb_launch_count()
     cams = rigs.yaw_ring(1, 64, 48, 70, 0)
     w = Warper()

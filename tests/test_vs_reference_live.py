@@ -1,231 +1,108 @@
-"""The oracle against the UNMODIFIED reference classes, live (build container only: needs /root/reference and cv2).
+"""The oracle and the drop-in classes against the UNMODIFIED reference classes on seeded random cases.
 
-The committed goldens (tests/golden/*.npz) were written by the reference once; this file re-derives the pin on random inputs (a fixed
-seed by default, SB_FUZZ_SEED=random for fresh ones), so that "the oracle is pinned" stays a checked statement wherever the
-reference can be imported:
+The committed goldens (tests/golden/*.npz) were written by the reference once; this file adds a wider pin on random inputs
+(tests/reference_cases.py, what the reference returned for them in tests/golden/golden_reference.npz):
 every projection of Warper.WARP_TYPE_CHOICES (roi, warped image, warped mask), the three blenders with gray and binary masks,
-and the Timelapser.  On the GPU box (no reference) the whole file skips; the goldens carry the pin there.
+the Timelapser, the FINAL-resolution steps, and the product's own classes side by side with the reference's.
 """
-import importlib
-import os
-import sys
-
 import numpy as np
 import pytest
 
-import replay
-from stitching_b200 import rigs
-
-REF = "/root/reference"
+import reference_cases as rc
+from stitching_b200 import Warper
 
 
 @pytest.fixture(scope="module")
-def ref():
-    pytest.importorskip("cv2")
-    if not os.path.isdir(os.path.join(REF, "stitching")):
-        pytest.skip("the reference checkout is not on this box")
-    sys.path.insert(0, REF)
-    for name in [m for m in sys.modules if m == "stitching" or m.startswith("stitching.")]:
-        del sys.modules[name]
-    mod = importlib.import_module("stitching")
-    importlib.import_module("stitching.warper")
-    importlib.import_module("stitching.blender")
-    importlib.import_module("stitching.timelapser")
-    yield mod
-    for name in [m for m in sys.modules if m == "stitching" or m.startswith("stitching.")]:
-        del sys.modules[name]
-    sys.path.remove(REF)
+def pins():
+    return rc.Pins()
 
 
-def _rng():
-    """Seeded for a reproducible suite; SB_FUZZ_SEED=random draws a fresh seed per run (printed, so that a failing draw can
-    be replayed with SB_FUZZ_SEED=<seed>) -- 150+ such runs went through without a difference while this file was written."""
-    env = os.environ.get("SB_FUZZ_SEED", "20260923")
-    seed = int.from_bytes(os.urandom(4), "little") if env == "random" else int(env)
-    print(f"SB_FUZZ_SEED={seed}")
-    return np.random.default_rng(seed)
-
-
-def _rot(rx, ry, rz):
-    cz, sz = np.cos(rz), np.sin(rz)
-    Rz = np.array([[cz, -sz, 0], [sz, cz, 0], [0, 0, 1]])
-    return (Rz @ rigs.rot_y(ry) @ rigs.rot_x(rx)).astype(np.float32)
-
-
-def test_every_projection_against_the_reference_warper(ref, oracle):
-    rng = _rng()
-    W, H = 88, 66
-    types = ref.warper.Warper.WARP_TYPE_CHOICES
-    assert len(types) == 16
+def test_every_projection_against_the_reference_warper(pins, oracle):
     checked = 0
-    for wtype in types:
-        for trial in range(3):
-            if wtype == "affine":
-                th, s = rng.uniform(-0.2, 0.2), rng.uniform(0.85, 1.2)
-                R = np.array([[s * np.cos(th), -s * np.sin(th), rng.uniform(-90, 300)], [s * np.sin(th), s * np.cos(th), rng.uniform(-40, 40)],
-                              [0, 0, 1]], np.float32)
-                cam, scale = rigs.Camera(1.0, 1.0, 0.0, 0.0, R), 1.0
-            else:
-                wide = wtype in ("spherical", "cylindrical")
-                R = _rot(rng.uniform(-0.3, 0.3), rng.uniform(-3.0, 3.0) if wide else rng.uniform(-0.45, 0.45), rng.uniform(-0.15, 0.15))
-                cam = rigs.Camera(rng.uniform(70, 120), rng.uniform(0.97, 1.03), W / 2 + rng.uniform(-4, 4), H / 2 + rng.uniform(-3, 3), R)
-                scale = float(rng.uniform(60, 120))
-            aspect = float(rng.choice([1.0, 0.8, 1.25])) if trial == 2 else 1.0
-            img = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
-            wr = ref.warper.Warper(wtype)
-            wr.scale = scale
-            K = ref.warper.Warper.get_K(cam, aspect)
-            roi = tuple(int(v) for v in wr.warp_roi((W, H), cam, aspect))
-            got_roi = oracle.warp_roi(wtype, scale * aspect, K, cam.R, (W, H))
-            assert tuple(got_roi) == roi, (wtype, trial, got_roi, roi)
-            if roi[2] * roi[3] > 4_000_000:
-                continue  # a degenerate draw (horizon in view): the rect is exact, the pixels would take minutes
-            rect, gimg, gmask = oracle.warp(wtype, scale * aspect, K, cam.R, img)
-            replay.assert_exact(gimg, wr.warp_image(img, cam, aspect), f"{wtype} trial {trial}: warped image")
-            replay.assert_exact(gmask, wr.create_and_warp_mask((W, H), cam, aspect), f"{wtype} trial {trial}: warped mask")
-            checked += 1
+    for key, wtype, cam, scale, aspect, img in rc.warp_cases():
+        K = Warper.get_K(cam, aspect)
+        size = (img.shape[1], img.shape[0])
+        roi = tuple(int(v) for v in pins.value(key + ".roi"))
+        got_roi = oracle.warp_roi(wtype, scale * aspect, K, cam.R, size)
+        assert tuple(got_roi) == roi, (key, got_roi, roi)
+        if roi[2] * roi[3] > 4_000_000:
+            continue  # a degenerate draw (horizon in view): the rect is exact, the pixels would take minutes
+        rect, gimg, gmask = oracle.warp(wtype, scale * aspect, K, cam.R, img)
+        pins.array(key + ".img", gimg, f"{key}: warped image")
+        pins.array(key + ".mask", gmask, f"{key}: warped mask")
+        checked += 1
     assert checked >= 40
 
 
-def test_blenders_and_timelapser_against_the_reference(ref, oracle):
-    rng = _rng()
-    for trial in range(9):
-        kind = ("multiband", "feather", "no")[trial % 3]
-        strength = float(rng.choice([1, 5, 20, 60]))
-        n = int(rng.integers(2, 5))
-        sizes = [(int(rng.integers(40, 120)), int(rng.integers(30, 90))) for _ in range(n)]
-        corners = [(int(rng.integers(-20, 20)) + 35 * i, int(rng.integers(-15, 15))) for i in range(n)]
-        imgs = [rng.integers(0, 256, (h, w, 3), dtype=np.uint8) for (w, h) in sizes]
-        masks = []
-        for (w, h) in sizes:
-            m = np.full((h, w), 255, np.uint8)
-            if trial % 2:
-                m[rng.random((h, w)) < 0.1] = 0
-            if trial % 4 == 3:
-                m = (m.astype(np.float32) * rng.random((h, w))).astype(np.uint8)  # gray seam-like masks
-            masks.append(m)
-        a, b = ref.blender.Blender(kind, strength), oracle.Blender(kind, strength)
-        a.prepare(corners, sizes)
+def test_blenders_and_timelapser_against_the_reference(pins, oracle):
+    for trial, kind, strength, corners, sizes, imgs, masks in rc.blend_cases():
+        b = oracle.Blender(kind, strength)
         b.prepare(corners, sizes)
         for img, m, c in zip(imgs, masks, corners):
-            a.feed(img, m, c)
             b.feed(img, m, c)
-        (pa, ma), (pb, mb) = a.blend(), b.blend()
-        replay.assert_exact(np.asarray(pb), np.asarray(pa), f"{kind} strength {strength}: panorama")
-        replay.assert_exact(np.asarray(mb), np.asarray(ma.get() if hasattr(ma, "get") else ma), f"{kind} strength {strength}: mask")
+        pb, mb = b.blend()
+        pins.array(f"blend.{trial}.pano", np.asarray(pb), f"{kind} strength {strength}: panorama")
+        pins.array(f"blend.{trial}.mask", np.asarray(mb), f"{kind} strength {strength}: mask")
         for tl_kind in ("as_is", "crop"):
-            ta, tb = ref.timelapser.Timelapser(tl_kind), oracle.Timelapser(tl_kind)
-            ta.initialize(corners, sizes)
+            tb = oracle.Timelapser(tl_kind)
             tb.initialize(corners, sizes)
-            for img, c in zip(imgs, corners):
-                ta.process_frame(img, c)
+            for i, (img, c) in enumerate(zip(imgs, corners)):
                 tb.process_frame(img, c)
+                key = f"timelapse.{trial}.{tl_kind}.{i}"
                 if tb.roi[2] == 0 or tb.roi[3] == 0:  # rects that touch in a line: the reference's get_frame raises on the empty canvas
-                    import cv2
-
-                    with pytest.raises(cv2.error):
-                        ta.get_frame()
+                    assert str(pins.value(key)) == "raises cv2.error", key
                     continue
-                replay.assert_exact(tb.get_frame(), ta.get_frame(), f"timelapse {tl_kind}")
+                pins.array(key, tb.get_frame(), f"timelapse {tl_kind}")
 
 
-def test_final_resolution_steps_against_the_reference(ref, oracle):
-    """SeamFinder.resize (seam_finder.py:38-43) and Images.resize_img_by_scaler (images.py:120-123) on fresh random shapes;
+def test_final_resolution_steps_against_the_reference(pins, oracle):
+    """SeamFinder.resize (seam_finder.py:38-43) and Images.resize_img_by_scaler (images.py:120-123) on random shapes;
     ExposureErrorCompensator.apply (exposure_error_compensator.py:43-45) with gains the reference's own feed() estimated."""
-    import cv2 as cv
-
-    importlib.import_module("stitching.seam_finder")
-    importlib.import_module("stitching.images")
-    importlib.import_module("stitching.exposure_error_compensator")
-    rng = _rng()
-    for t in range(10):
-        sh, sw = int(rng.integers(1, 70)), int(rng.integers(1, 90))
-        h, w = int(rng.integers(2, 300)), int(rng.integers(2, 400))
-        seam = (rng.integers(0, 256, (sh, sw), dtype=np.uint8) if t % 2 else (rng.random((sh, sw)) < 0.5).astype(np.uint8) * 255)
-        mask = (rng.random((h, w)) < 0.85).astype(np.uint8) * 255
-        want = ref.seam_finder.SeamFinder.resize(cv.UMat(seam), mask)
-        replay.assert_exact(oracle.seam_resize(seam, mask), want.get() if hasattr(want, "get") else np.asarray(want), f"SeamFinder.resize {sw}x{sh} -> {w}x{h}")
-
-    class Scaler:
-        def __init__(self, size):
-            self.size = size
-
-        def get_scaled_img_size(self, _):
-            return self.size
-
-    for t in range(10):
-        h, w = int(rng.integers(2, 200)), int(rng.integers(2, 260))
-        size = (int(rng.integers(1, 300)), int(rng.integers(1, 240)))
-        img = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
-        want = ref.images.Images.resize_img_by_scaler(Scaler(size), (w, h), img)
-        replay.assert_exact(oracle.resize_linear_exact(img, size), want, f"Images.resize {w}x{h} -> {size}")
-
-    kinds = ref.exposure_error_compensator.ExposureErrorCompensator.COMPENSATOR_CHOICES
-    for t, kind in enumerate(kinds):
-        n = 3
-        sizes = [(int(rng.integers(90, 160)), int(rng.integers(70, 120))) for _ in range(n)]
-        corners = [(40 * i + int(rng.integers(-5, 5)), int(rng.integers(-5, 5))) for i in range(n)]
-        base = rng.integers(30, 220, (200, 400, 3), dtype=np.uint8)
-        imgs = []
-        for i, ((w, h), (x, y)) in enumerate(zip(sizes, corners)):
-            crop = base[20 + y: 20 + y + h, 20 + x: 20 + x + w].astype(np.float32) * (0.8 + 0.2 * i)
-            imgs.append(np.clip(crop + rng.normal(0, 2, crop.shape), 0, 255).astype(np.uint8))
-        masks = [np.full((h, w), 255, np.uint8) for (w, h) in sizes]
-        comp = ref.exposure_error_compensator.ExposureErrorCompensator(kind, 1, 16)
-        comp.feed(corners, imgs, masks)
-        for i in range(n):
-            want = comp.apply(i, corners[i], imgs[i].copy(), masks[i])
-            if kind == "no":
-                replay.assert_exact(imgs[i], want, "compensator no: identity")
-                continue
-            gain = np.asarray(comp.compensator.getMatGains()[i])
-            replay.assert_exact(oracle.gain_apply(imgs[i], gain), want, f"compensator {kind} image {i}")
+    for case in rc.final_resolution_cases():
+        if case[0] == "seam":
+            _, t, seam, mask = case
+            pins.array(f"seam.{t}", oracle.seam_resize(seam, mask), f"SeamFinder.resize {seam.shape} -> {mask.shape}")
+        elif case[0] == "resize":
+            _, t, img, size = case
+            pins.array(f"resize.{t}", oracle.resize_linear_exact(img, size), f"Images.resize {img.shape} -> {size}")
+        else:
+            _, kind, corners, imgs, masks = case
+            for i in range(len(imgs)):
+                if kind == "no":
+                    pins.array(f"gain.no.{i}", imgs[i], "compensator no: identity")
+                    continue
+                gain = pins.value(f"gain.{kind}.{i}.gains")
+                pins.array(f"gain.{kind}.{i}", oracle.gain_apply(imgs[i], gain), f"compensator {kind} image {i}")
 
 
-def test_drop_in_classes_against_the_reference_classes(ref, use_emu):
-    """The product's own classes (their kernels through tests/emu) side by side with the reference's, same calls, same inputs:
+def test_drop_in_classes_against_the_reference_classes(pins, use_emu):
+    """The product's own classes (their kernels through tests/emu) against the reference's, same calls, same inputs:
     Warper (set_scale, warp_rois, warp_images, create_and_warp_masks) -> Blender (prepare, feed, blend) for random rigs of every
     blender type and a handful of projections, and Timelapser frames of the same warped images."""
     import stitching_b200
 
-    rng = _rng()
-    W, H = 120, 90
-    for trial, (wtype, btype) in enumerate((("spherical", "multiband"), ("cylindrical", "feather"), ("plane", "no"), ("fisheye", "multiband"),
-                                            ("paniniA2B1", "feather"), ("mercator", "multiband"), ("affine", "multiband"))):
-        n = 3
-        if wtype == "affine":
-            cams = [rigs.Camera(1.0, 1.0, 0.0, 0.0, np.array([[1, 0.01 * i, 70.0 * i + rng.uniform(-3, 3)], [-0.01 * i, 1, rng.uniform(-8, 8)], [0, 0, 1]], np.float32))
-                    for i in range(n)]
-        else:
-            f = rng.uniform(90, 130)
-            cams = [rigs.Camera(f * rng.uniform(0.98, 1.02), 1.0, W / 2, H / 2, _rot(rng.uniform(-0.05, 0.05), 0.45 * (i - 1) + rng.uniform(-0.03, 0.03), rng.uniform(-0.03, 0.03)))
-                    for i in range(n)]
-        imgs = [rng.integers(0, 256, (H, W, 3), dtype=np.uint8) for _ in range(n)]
-        sizes = [(W, H)] * n
-        out = []
-        for Warper, Blender, Timelapser in ((ref.warper.Warper, ref.blender.Blender, ref.timelapser.Timelapser),
-                                            (stitching_b200.Warper, stitching_b200.Blender, stitching_b200.Timelapser)):
-            w = Warper(wtype)
-            w.set_scale(cams)
-            warped = list(w.warp_images(imgs, cams))
-            masks = list(w.create_and_warp_masks(sizes, cams))
-            corners, wsizes = w.warp_rois(sizes, cams)
-            b = Blender(btype, 5)
-            b.prepare(corners, wsizes)
-            for img, m, c in zip(warped, masks, corners):
-                b.feed(img, m, c)
-            pano, pmask = b.blend()
-            t = Timelapser("as_is")
-            t.initialize(corners, wsizes)
-            t.process_frame(warped[1], corners[1])
-            out.append(dict(corners=[tuple(int(v) for v in c) for c in corners], sizes=[tuple(int(v) for v in s) for s in wsizes],
-                            warped=[np.asarray(x) for x in warped], masks=[np.asarray(x) for x in masks], pano=np.asarray(pano),
-                            pmask=np.asarray(pmask.get() if hasattr(pmask, "get") else pmask), frame=np.asarray(t.get_frame())))
-        a, b = out
-        assert a["corners"] == b["corners"] and a["sizes"] == b["sizes"], (wtype, a["corners"], b["corners"])
-        for i in range(n):
-            replay.assert_exact(b["warped"][i], a["warped"][i], f"{wtype}: warped image {i}")
-            replay.assert_exact(b["masks"][i], a["masks"][i], f"{wtype}: warped mask {i}")
-        replay.assert_exact(b["pano"], a["pano"], f"{wtype} + {btype}: panorama")
-        replay.assert_exact(b["pmask"], a["pmask"], f"{wtype} + {btype}: panorama mask")
-        replay.assert_exact(b["frame"], a["frame"], f"{wtype}: timelapse frame")
+    for trial, wtype, btype, cams, imgs in rc.dropin_cases():
+        key = f"dropin.{trial}"
+        sizes = [(img.shape[1], img.shape[0]) for img in imgs]
+        w = stitching_b200.Warper(wtype)
+        w.set_scale(cams)
+        warped = list(w.warp_images(imgs, cams))
+        masks = list(w.create_and_warp_masks(sizes, cams))
+        corners, wsizes = w.warp_rois(sizes, cams)
+        b = stitching_b200.Blender(btype, 5)
+        b.prepare(corners, wsizes)
+        for img, m, c in zip(warped, masks, corners):
+            b.feed(img, m, c)
+        pano, pmask = b.blend()
+        t = stitching_b200.Timelapser("as_is")
+        t.initialize(corners, wsizes)
+        t.process_frame(warped[1], corners[1])
+        got = [[tuple(int(v) for v in c) for c in corners], [tuple(int(v) for v in s) for s in wsizes]]
+        want = [[tuple(int(v) for v in c) for c in pins.value(key + ".corners")], [tuple(int(v) for v in s) for s in pins.value(key + ".sizes")]]
+        assert got == want, (wtype, got, want)
+        for i in range(len(imgs)):
+            pins.array(f"{key}.warped.{i}", warped[i], f"{wtype}: warped image {i}")
+            pins.array(f"{key}.mask.{i}", masks[i], f"{wtype}: warped mask {i}")
+        pins.array(key + ".pano", pano, f"{wtype} + {btype}: panorama")
+        pins.array(key + ".pmask", pmask, f"{wtype} + {btype}: panorama mask")
+        pins.array(key + ".frame", t.get_frame(), f"{wtype}: timelapse frame")
