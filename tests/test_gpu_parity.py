@@ -172,8 +172,11 @@ def test_blend_fuzz_against_oracle(cuda_lib, oracle):
             o.feed(img, m, c)
             b.feed(img, m, c)
         os16, om = o.blend_s16()
-        pano, pmask, s16 = b.blender.blend(want_s16=True)
-        assert_parity(s16, os16, f"blend fuzz {t} {btype} int16 result")
+        if t % 4 in (0, 3):
+            pano, pmask, s16 = b.blender.blend(want_s16=True)
+            assert_parity(s16, os16, f"blend fuzz {t} {btype} int16 result")
+        else:  # uint8 result only: level 0 of the collapse may run in the tile kernel (it never writes int16)
+            pano, pmask = b.blender.blend()
         assert_parity(pano, oracle.convert_scale_abs(os16), f"blend fuzz {t} {btype} uint8 result")
         assert np.array_equal(pmask, om), f"blend fuzz {t} {btype} mask"
 

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 import replay
+import rig_fuzz
 from stitching_b200 import Blender, Compositor, StitchingError, Warper, rigs
 
 
@@ -531,3 +532,37 @@ def _compositor_other_projections(oracle, names):
 
 def test_compositor_with_the_other_projections(use_emu, oracle):
     _compositor_other_projections(oracle, ["fisheye", "compressedPlaneA2B1", "paniniPortraitA1.5B1", "mercator", "transverseMercator", "stereographic"])
+
+
+# -- seeded random rigs (tests/rig_fuzz.py) through the emulation build, bit for bit against the oracle -------------------
+_EMU_SEED = rig_fuzz.seed_from_env()
+
+
+@pytest.mark.parametrize("k", range(len(rig_fuzz.emu_ids())), ids=rig_fuzz.emu_ids())
+def test_rig_fuzz_against_oracle(use_emu, oracle, monkeypatch, k):
+    """One random rig (or one named rig that aims at a branch): rects, pano roi, num_bands, every warped image and mask,
+    the panorama and its mask equal the oracle's.  The named cases run the shuffle pyrDown (SB_EMU_LANES) or the tile
+    collapse (SB_EMU_BLOCKS) of the emulation build."""
+    case = rig_fuzz.emu_set(_EMU_SEED)[k]
+    for key, v in case.env.items():
+        monkeypatch.setenv(key, v)
+    imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(case)
+    ref = rig_fuzz.oracle_run(oracle, case, imgs, ex)
+    got = rig_fuzz.compositor_run(Compositor, case, imgs, ex)
+    rig_fuzz.check(case, got, ref, _EMU_SEED)
+
+
+def test_rig_fuzz_coverage_under_emulation(oracle):
+    """The emulated fuzz set reaches the branches the emulation build can run, by the launchers' own predicates."""
+    cs = rig_fuzz.emu_set(_EMU_SEED)
+    rows = [(c, rig_fuzz.emu_coverage(c)) for c in cs]
+    print(f"\nrig fuzz coverage, emulation set (seed {_EMU_SEED}, {len(cs)} cases):\n" + rig_fuzz.coverage_table(rows))
+    reached = set().union(*(t for _, t in rows))
+    want = {"nb=0", "nb=1", "nb>=2", "feather", "no", "n>32", "odd pano width", "map projection", "mixed extras",
+            "gray blend mask", "k_warp_rgbm<HAS_BM=1>", "k_warp_rgbm<HAS_BM=0>", "tile l0 yes", "tile l0 no",
+            "k_pyrdown_walk<1,0,1>", "k_pyrdown_walk<0,1,1>", "k_pyrdown_walk<0,0,0>", "k_pyrdown_walk<1,1,0>"}
+    assert want <= reached, f"not reached: {sorted(want - reached)}"
+    lanes_gray = [c for c in cs if "SB_EMU_LANES" in c.env and c.blender == "multiband" and
+                  any(m in ("ramp", "random") for m in c.masks)]
+    assert lanes_gray, "a gray set_mask must run through the shuffle pyrDown (BIN off)"
+    assert rig_fuzz.redraw_share(cs) < 0.5, f"{rig_fuzz.redraw_share(cs):.2f} rejected draws per case"
