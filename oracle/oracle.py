@@ -65,6 +65,8 @@ def lib():
         L.so_sb_destroy.restype = None
         L.so_sb_feed.argtypes = [C.c_void_p, s16p, C.c_size_t, u8p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int]
         L.so_sb_blend.argtypes = [C.c_void_p, s16p, u8p]
+        L.so_mb_fold.argtypes = [C.c_void_p, C.c_void_p]
+        L.so_sb_fold.argtypes = [C.c_void_p, C.c_void_p]
         L.so_convert_scale_abs_s16.argtypes = [s16p, C.c_size_t, u8p]
         L.so_resize_linear_f32.argtypes = [fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, fp]
         L.so_resize_linear_exact_u8.argtypes = [u8p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, u8p]
@@ -339,6 +341,16 @@ class Blender:
         rc = f(self._h, _p(img, C.c_int16), w * 3, _p(mask, C.c_uint8), w, w, h, int(corner[0]), int(corner[1]))
         if rc:
             raise ValueError("feed rect outside the prepared roi")
+
+    def fold(self, other):
+        """Add `other`'s accumulators into this blender's (int16 sums with wrap-around, float weight sums with a plain
+        +=); `other` must be prepared with the same roi and kind and is left as it was.  Restates how the owner of a
+        strip in the sharded composite adds another rank's partial sums."""
+        if self._kind != other._kind or self.roi != other.roi or self._kind == "no":
+            raise ValueError("fold needs two multiband or two feather blenders prepared with the same roi")
+        f = lib().so_mb_fold if self._kind == "multiband" else lib().so_sb_fold
+        if f(self._h, other._h):
+            raise ValueError("fold: blenders of different geometry")
 
     def blend_s16(self):
         x, y, w, h = self.roi

@@ -648,6 +648,22 @@ SO_API int so_mb_feed(void *hnd, const int16_t *img, size_t img_pitch_elems, con
     return 0;
 }
 
+/* dst's accumulators += src's, level by level: int16 with wrap-around, float weights with a plain +=.  src is not
+ * consumed.  Test infrastructure for the sharded composite, whose strip owner adds other ranks' partial sums in these
+ * groups (sb_shard.cpp); -1 when the two blenders were prepared with different geometry. */
+SO_API int so_mb_fold(void *dst_h, const void *src_h)
+{
+    so_mb *d = (so_mb *)dst_h;
+    const so_mb *s = (const so_mb *)src_h;
+    if (d->nb != s->nb || d->x != s->x || d->y != s->y || d->w != s->w || d->h != s->h) return -1;
+    for (int l = 0; l <= d->nb; ++l) {
+        size_t n = (size_t)d->lw[l] * d->lh[l];
+        for (size_t i = 0; i < n * 3; ++i) d->lap[l][i] = (int16_t)(d->lap[l][i] + s->lap[l][i]);
+        for (size_t i = 0; i < n; ++i) d->wt[l][i] += s->wt[l][i];
+    }
+    return 0;
+}
+
 /* blend(): dst int16x3 [h][w], dst_mask u8 [h][w]  (consumes the accumulators) */
 SO_API int so_mb_blend(void *hnd, int16_t *dst, uint8_t *dst_mask)
 {
@@ -761,6 +777,19 @@ SO_API int so_sb_feed(void *hnd, const int16_t *img, size_t img_pitch_elems, con
     free(wm);
     return 0;
 }
+/* feather: dst's accumulators += src's (int16 with wrap-around, float weights with a plain +=); src is not consumed.
+ * -1 for the NO blender (its feed overwrites, there is nothing to add) or a different geometry. */
+SO_API int so_sb_fold(void *dst_h, const void *src_h)
+{
+    so_sb *d = (so_sb *)dst_h;
+    const so_sb *s = (const so_sb *)src_h;
+    if (d->kind != 1 || s->kind != 1 || d->x != s->x || d->y != s->y || d->w != s->w || d->h != s->h) return -1;
+    size_t n = (size_t)d->w * d->h;
+    for (size_t i = 0; i < n * 3; ++i) d->acc[i] = (int16_t)(d->acc[i] + s->acc[i]);
+    for (size_t i = 0; i < n; ++i) d->wsum[i] += s->wsum[i];
+    return 0;
+}
+
 SO_API int so_sb_blend(void *hnd, int16_t *dst, uint8_t *dst_mask)
 {
     so_sb *b = (so_sb *)hnd;

@@ -7,9 +7,10 @@
 // its partial sums (acc int16x3 with wrap-around, wsum float32) over the part of the strip -- plus a 2-pixel
 // margin per level, which is what the pyrUp of the next finer level reads -- that its footprint covers.  The owner
 // adds the slabs and its own images in rank order inside the ordinary per-level kernel and collapses its strip.
-// int16 wrap-around sums are exact under any grouping; the float weight sums are grouped per rank, which is
-// bit-identical to the single-GPU order whenever at most two ranks meet in a pixel with at most one image each
-// and otherwise differs by float re-association only (tests bound the effect on the final uint8 to +-1).
+// int16 wrap-around sums are exact under any grouping; the float weight sums are grouped per rank (each slab a sum
+// from 0, added in rank order around the owner's own images), which can differ from the single-GPU order by float
+// re-association.  The grouping is deterministic: tests/shard_fuzz.py restates it with the CPU oracle
+// (oracle.Blender.fold) and the tests compare every strip with it bit for bit.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -136,7 +137,9 @@ int ShardPlan::build(const BlendPlan &plan, int rank_, int world_)
     reversed = false;
     block_of(n, world, rank, &first, &count);
     if (plan.kind == SB_BLEND_FEATHER) return build_feather(plan);
-    // strip boundaries: halfway between the centres of the neighbouring blocks' edge images, snapped to 2^nb
+    // strip boundaries: halfway between the centres of the neighbouring blocks' edge images, snapped to 2^nb.  Blocks
+    // that run right to left would give decreasing boundaries: refused rather than clamped, which would leave one rank
+    // the whole panorama and the others nothing.  Equal boundaries (an empty strip) are fine.
     const int a = 1 << plan.nb;
     bounds.assign(world + 1, 0);
     bounds[world] = plan.wp;
@@ -146,16 +149,14 @@ int ShardPlan::build(const BlendPlan &plan, int rank_, int world_)
         block_of(n, world, r, &g0, &gc);
         const FeedImage &L = plan.imgs[f0 + fc - 1], &R = plan.imgs[g0];
         const long long mid = ((long long)L.px + L.left + L.w / 2 + R.px + R.left + R.w / 2) / 2;
-        int b = (int)((mid + a / 2) / a * a);
-        b = std::max(b, bounds[r - 1]);
-        b = std::min(b, plan.wp);
-        bounds[r] = b;
-    }
-    for (int r = 1; r <= world; ++r)
-        if (bounds[r] < bounds[r - 1]) {
-            set_error("sharded composite: image blocks are not ordered left to right in the panorama");
+        const int b = (int)std::min<long long>((mid + a / 2) / a * a, plan.wp);
+        if (b < bounds[r - 1]) {
+            set_error("sharded composite: image blocks are not ordered left to right in the panorama (boundary %d at column %d, "
+                      "boundary %d at column %d)", r - 1, bounds[r - 1], r, b);
             return SB_ERR_INVALID;
         }
+        bounds[r] = b;
+    }
     send.assign(world, PeerSlab());
     recv.assign(world, PeerSlab());
     for (int p = 0; p < world; ++p) {

@@ -4,11 +4,10 @@ Needs >= 2 GPUs on the box (gpurun --gpus 2); on a 1-GPU box the test is skipped
 covered by tests/test_gpu_parity.py::test_sharded_roles_on_one_gpu and the host logic by tests/test_sharded.py.
 """
 import os
-import subprocess
-import sys
 
 import pytest
 
+import torchrun_job
 from conftest import ROOT
 
 pytestmark = pytest.mark.gpu
@@ -40,13 +39,14 @@ if rank == 0:
     ax = 0 if c.strip_axis else 1
     full = np.concatenate([p[1] for p in parts], axis=ax)
     fmask = np.concatenate([p[2] for p in parts], axis=ax)
-    single = Compositor(cams, sizes, cfg["warper"], cfg["blender"], cfg["strength"])
-    ref, rmask = single.composite(imgs)
-    d = np.abs(full.astype(np.int32) - ref.astype(np.int32))
+    # the oracle summed in the ranks' groups (tests/shard_fuzz.py), bit for bit
+    sys.path.insert(0, os.path.join(sys.argv[1], "tests"))
+    import shard_fuzz
+    from oracle import oracle as O
+    ref, rmask, _ = shard_fuzz.grouped_panorama(O, shard_fuzz.config_case(cfg, world, cams), imgs)
     assert full.shape == ref.shape and np.array_equal(fmask, rmask), (full.shape, ref.shape)
-    assert d.max() <= 1, int(d.max())
-    print("SHARDED_OK", name, world, "ranks; differing values:", int((d != 0).sum()), "of", d.size, "; step ms", ms / 5,
-          dict((k, round(v, 3)) for k, v in launches))
+    assert np.array_equal(full, ref), int((full != ref).sum())
+    print("SHARDED_OK", name, world, "ranks; step ms", ms / 5, dict((k, round(v, 3)) for k, v in launches))
 c.close()
 sbdist.shutdown()
 dist.destroy_process_group()
@@ -71,9 +71,8 @@ def test_nccl_sharded_composite(tmp_path, name, scale_down, n_images):
     world = 2 if n < 4 else 4
     script = tmp_path / "worker.py"
     script.write_text(WORKER)
-    out = subprocess.run(
-        [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-         "--master-port", "29621", str(script), ROOT, name, str(scale_down), str(n_images)],
-        capture_output=True, text=True, timeout=900, env=dict(os.environ, MASTER_ADDR="127.0.0.1"))
-    print(out.stdout[-1500:])
-    assert out.returncode == 0 and "SHARDED_OK" in out.stdout, out.stdout[-3000:] + out.stderr[-3000:]
+    out = torchrun_job.run(world, 29621, script, [ROOT, name, scale_down, n_images], dict(os.environ, MASTER_ADDR="127.0.0.1"),
+                           timeout=900)
+    print(out["stdout"][-1500:])
+    assert not out["timed_out"] and not out["leftover"], out["stdout"][-3000:] + out["stderr"][-3000:]
+    assert out["returncode"] == 0 and "SHARDED_OK" in out["stdout"], out["stdout"][-3000:] + out["stderr"][-3000:]

@@ -6,13 +6,13 @@ real GPUs by tests/test_gpu_sharded.py.
 """
 import ctypes as C
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 import replay
+import shard_fuzz
+import torchrun_job
 from conftest import ROOT
 from stitching_b200 import Compositor, rigs
 
@@ -51,65 +51,52 @@ def run_sharded(cfg, cams, imgs, world, copy):
     return pano, mask, moved
 
 
+def assert_grouped(oracle, cfg, cams, imgs, world, pano, mask):
+    """The strips put together equal the oracle summed in the ranks' groups (tests/shard_fuzz.py) bit for bit: the
+    int16 sums are exact under any grouping and the float weight sums are grouped as the ranks group them.  Returns
+    the oracle's num_bands."""
+    ref_pano, ref_mask, nb = shard_fuzz.grouped_panorama(oracle, shard_fuzz.config_case(cfg, world, cams), imgs)
+    replay.assert_exact(mask, ref_mask, f"sharded x{world} mask")
+    replay.assert_exact(pano, ref_pano, f"sharded x{world} pano")
+    return nb
+
+
 @pytest.mark.parametrize("world", [2, 3, 4])
-def test_sharded_equals_single(use_emu, oracle, world):
+def test_sharded_equals_grouped_oracle(use_emu, oracle, world):
     cfg = rigs.config("cfg2", 16)
     cams = cfg["cameras"]
     imgs = [rigs.noise_image(cfg["h"], cfg["w"], 70 + i) if i % 2 else rigs.synth_image(cfg["h"], cfg["w"], 70 + i) for i in range(len(cams))]
-    single = Compositor(cams, [(cfg["w"], cfg["h"])] * len(cams), cfg["warper"], cfg["blender"], cfg["strength"])
-    ref_pano, ref_mask = single.composite(imgs)
-    assert single.num_bands >= 2
-    single.close()
     pano, mask, moved = run_sharded(cfg, cams, imgs, world, lambda d, s, n: C.memmove(d, s, n))
     assert moved > 0
-    assert np.array_equal(mask, ref_mask)
-    d = np.abs(pano.astype(np.int32) - ref_pano.astype(np.int32))
-    # int16 sums are exact under regrouping; the float weight sums are regrouped per rank: at most +-1 in the uint8
-    assert d.max() <= 1, int(d.max())
-    assert (d != 0).mean() < 1e-3
+    assert assert_grouped(oracle, cfg, cams, imgs, world, pano, mask) >= 2
 
 
-def test_sharded_cylindrical_many_images(use_emu):
+def test_sharded_cylindrical_many_images(use_emu, oracle):
     cfg = rigs.config("cfg3", 20)  # 32 images, cylindrical (BASELINE configs[2] layout: 4 images per rank at world 8)
     cams = cfg["cameras"]
     imgs = [rigs.synth_image(cfg["h"], cfg["w"], 5 + i) for i in range(len(cams))]
-    single = Compositor(cams, [(cfg["w"], cfg["h"])] * len(cams), cfg["warper"], cfg["blender"], cfg["strength"])
-    ref_pano, ref_mask = single.composite(imgs)
-    single.close()
     pano, mask, _ = run_sharded(cfg, cams, imgs, 8, lambda d, s, n: C.memmove(d, s, n))
-    assert np.array_equal(mask, ref_mask)
-    assert np.abs(pano.astype(np.int32) - ref_pano.astype(np.int32)).max() <= 1
+    assert_grouped(oracle, cfg, cams, imgs, 8, pano, mask)
 
 
 @pytest.mark.parametrize("world", [2, 4])
-def test_sharded_feather_grid(use_emu, world):
+def test_sharded_feather_grid(use_emu, oracle, world):
     """BASELINE configs[4]: 4x4 plane grid, feather blender; image blocks are grid rows, so the ranks own ROW strips."""
     cfg = rigs.config("cfg5", 12)
     cams = cfg["cameras"]
     imgs = [rigs.noise_image(cfg["h"], cfg["w"], 30 + i) if i % 3 == 0 else rigs.synth_image(cfg["h"], cfg["w"], 30 + i) for i in range(len(cams))]
-    single = Compositor(cams, [(cfg["w"], cfg["h"])] * len(cams), cfg["warper"], cfg["blender"], cfg["strength"])
-    ref_pano, ref_mask = single.composite(imgs)
-    single.close()
     pano, mask, moved = run_sharded(cfg, cams, imgs, world, lambda d, s, n: C.memmove(d, s, n))
     assert moved > 0
-    assert pano.shape == ref_pano.shape
-    assert np.array_equal(mask, ref_mask)
-    d = np.abs(pano.astype(np.int32) - ref_pano.astype(np.int32))
-    assert d.max() <= 1, int(d.max())  # float sums regrouped per rank
-    assert (d != 0).mean() < 1e-3
+    assert_grouped(oracle, cfg, cams, imgs, world, pano, mask)
 
 
-def test_sharded_feather_side_by_side(use_emu):
+def test_sharded_feather_side_by_side(use_emu, oracle):
     """Feather on a single-row rig: the blocks lie side by side and the strips are columns, as for multiband."""
     cfg = dict(rigs.config("cfg2", 16), blender="feather")
     cams = cfg["cameras"]
     imgs = [rigs.synth_image(cfg["h"], cfg["w"], 11 + i) for i in range(len(cams))]
-    single = Compositor(cams, [(cfg["w"], cfg["h"])] * len(cams), cfg["warper"], "feather", cfg["strength"])
-    ref_pano, ref_mask = single.composite(imgs)
-    single.close()
     pano, mask, _ = run_sharded(cfg, cams, imgs, 2, lambda d, s, n: C.memmove(d, s, n))
-    assert np.array_equal(mask, ref_mask)
-    assert np.abs(pano.astype(np.int32) - ref_pano.astype(np.int32)).max() <= 1
+    assert_grouped(oracle, cfg, cams, imgs, 2, pano, mask)
 
 
 def test_sharded_rejects_what_it_cannot_do(use_emu):
@@ -157,8 +144,25 @@ def test_world_size_2_gloo_rendezvous_and_partition(emu_lib, tmp_path):
     script = tmp_path / "worker.py"
     script.write_text(GLOO_WORKER)
     env = dict(os.environ, MASTER_ADDR="127.0.0.1")
-    out = subprocess.run(
-        [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
-         "--master-port", "29613", str(script), ROOT],
-        capture_output=True, text=True, env=env, timeout=300)
-    assert out.returncode == 0 and "GLOO_OK" in out.stdout, out.stdout[-2000:] + out.stderr[-2000:]
+    out = torchrun_job.run(2, 29613, script, [ROOT], env, timeout=300)
+    assert not out["timed_out"] and not out["leftover"], out["stdout"][-2000:] + out["stderr"][-2000:]
+    assert out["returncode"] == 0 and "GLOO_OK" in out["stdout"], out["stdout"][-2000:] + out["stderr"][-2000:]
+
+
+STUCK_WORKER = r"""
+import signal, sys, time
+signal.signal(signal.SIGTERM, signal.SIG_IGN)   # a rank that does not stop when asked
+print("STARTED", flush=True)
+time.sleep(3600)
+"""
+
+
+def test_torchrun_job_timeout_leaves_no_process(tmp_path):
+    """The torchrun helper of the multi-GPU tests: a job that overruns its timeout is torn down -- the launcher and every
+    worker, also workers that ignore SIGTERM -- and reported as timed out (CPU only: the workers just sleep)."""
+    script = tmp_path / "stuck.py"
+    script.write_text(STUCK_WORKER)
+    out = torchrun_job.run(2, 29617, script, [], dict(os.environ, MASTER_ADDR="127.0.0.1"), timeout=15, grace=3)
+    assert out["timed_out"], out["stdout"][-2000:] + out["stderr"][-2000:]
+    assert out["stdout"].count("STARTED") == 2, out["stdout"][-2000:] + out["stderr"][-2000:]
+    assert out["leftover"] == []
