@@ -23,18 +23,25 @@ using namespace sb;
 
 #define SB_PIPE_DEPTH 3  // buffer sets of the pipelined submit / wait path
 
+// One buffer set.  Slot 0 serves upload / run / download, the timing calls and the sharded step; the pipelined
+// submit / wait path deals its steps round-robin to all SB_PIPE_DEPTH slots.
+struct Slot {
+    std::vector<uint8_t *> src;    // u8x3 sources as uploaded (null: an image of another rank)
+    std::vector<uint32_t *> src4;  // the same, one word per pixel: what the warp kernel reads (repacked after every upload)
+    PanoOut out{};                 // device outputs
+    cudaEvent_t e_h2d = nullptr, e_comp = nullptr, e_d2h = nullptr;  // submit: sources uploaded, step done, output downloaded
+#ifndef SB_EMU
+    cudaGraphExec_t graph = nullptr;  // the captured step reading this slot's buffers
+#endif
+};
+
 struct sb_compositor {
     int n = 0;
-    int warp_type = 0, blend_kind_requested = 0, mask_mode = 0;
-    float scale = 1.f, blend_strength = 5.f;
     cudaStream_t stream = nullptr;
     std::vector<int> src_w, src_h;
     std::vector<Rect> rects;           // warped rects (pano-absolute)
-    std::vector<WarpJob> jobs;         // host copy
-    std::vector<WarpJob> jobsx[SB_PIPE_DEPTH - 1];  // the same jobs reading the extra source buffer sets (pipelined path)
-    std::vector<uint8_t *> src_dev;    // u8x3 sources as uploaded
-    std::vector<uint32_t *> src4_dev;  // the same, one word per pixel: what the warp kernel reads (repacked after every upload)
-    std::vector<uint32_t *> src4_devx[SB_PIPE_DEPTH - 1];
+    std::vector<WarpJob> jobs;         // host copy, reading slot 0's sources
+    std::vector<WarpJob> slot_jobs;    // scratch: the jobs of another slot (slot_jobs_of)
     bool use_src4 = true;
     std::vector<uint32_t *> rgbm_dev;  // warped, packed; row pitch = width rounded up to 32 pixels (128-byte rows)
     std::vector<float *> tab_dev;
@@ -43,23 +50,16 @@ struct sb_compositor {
     std::vector<GainData> gain;        // exposure gains per image (sb_compositor_set_gain)
     int max_w = 0, max_h = 0;
     BlendPlan plan;
-    PanoOut out{};                     // device outputs
+    Slot slots[SB_PIPE_DEPTH];
+    int n_slots = 0;                   // slots with buffers: 1 from creation, all from the first submit on
     void *flush_buf = nullptr;
     size_t flush_bytes = 0;
     std::vector<cudaEvent_t> ev;       // ev[0] = start, ev[k+1] = after launch k
     std::vector<std::string> launch_names;
     std::vector<float> launch_ms;      // per launch, averaged over the last sb_compositor_time call
     double warp_bytes = 0;
-    // pipelined submit / wait: a second set of source + output buffers, copy streams, per-slot events
-    bool pipe_ready = false;
-    std::vector<uint8_t *> src_devx[SB_PIPE_DEPTH - 1];
-    PanoOut outx[SB_PIPE_DEPTH - 1] = {};
-    cudaStream_t h2d = nullptr, d2h = nullptr;
-    cudaEvent_t e_h2d[SB_PIPE_DEPTH] = {}, e_comp[SB_PIPE_DEPTH] = {}, e_d2h[SB_PIPE_DEPTH] = {};
+    cudaStream_t h2d = nullptr, d2h = nullptr;  // copy streams of the pipelined path
     unsigned long long submitted = 0;
-#ifndef SB_EMU
-    cudaGraphExec_t graph_exec[SB_PIPE_DEPTH] = {};  // one captured step per buffer slot
-#endif
     unsigned graph_kernels = 0;
     std::vector<cudaEvent_t> tev;  // step start / end events of sb_compositor_time
     // multi-GPU: this process composites images [first, first + count) and one column strip of the panorama
@@ -71,52 +71,63 @@ struct sb_compositor {
     ShardPlan shard;
 };
 
+// the sources of this rank's images and an output of slot 0's size (the panorama, or this rank's strip)
+static int slot_alloc(sb_compositor *c, Slot &sl)
+{
+    cudaStream_t s = c->stream;
+    sl.src.assign(c->n, nullptr);
+    sl.src4.assign(c->n, nullptr);
+    for (int i = c->first; i < c->first + c->count; ++i) {
+        const long long px = (long long)c->src_w[i] * c->src_h[i];
+        SB_TRY(dev_alloc((void **)&sl.src[i], (size_t)px * 3 + SB_SRC_PAD, s));
+        if (c->use_src4 && px < (1ll << 31)) SB_TRY(dev_alloc((void **)&sl.src4[i], ((size_t)px + 4) * sizeof(uint32_t), s));
+    }
+    PanoOut &o = sl.out;
+    o.w = c->slots[0].out.w;
+    o.h = c->slots[0].out.h;
+    o.rgb_pitch = (long long)o.w * 3;
+    o.mask_pitch = o.w;
+    SB_TRY(dev_alloc((void **)&o.rgb, (size_t)std::max(o.w, 1) * 3 * std::max(o.h, 1), s));
+    SB_TRY(dev_alloc((void **)&o.mask, (size_t)std::max(o.w, 1) * std::max(o.h, 1), s));
+    SB_CUDA(cudaEventCreateWithFlags(&sl.e_h2d, cudaEventDisableTiming));
+    SB_CUDA(cudaEventCreateWithFlags(&sl.e_comp, cudaEventDisableTiming));
+    SB_CUDA(cudaEventCreateWithFlags(&sl.e_d2h, cudaEventDisableTiming));
+    return SB_OK;
+}
+
+static void slot_free(Slot &sl, cudaStream_t s)
+{
+    for (auto p : sl.src) dev_free(p, s);
+    for (auto p : sl.src4) dev_free(p, s);
+    dev_free(sl.out.rgb, s);
+    dev_free(sl.out.mask, s);
+    for (cudaEvent_t e : {sl.e_h2d, sl.e_comp, sl.e_d2h})
+        if (e) (void)cudaEventDestroy(e);
+#ifndef SB_EMU
+    if (sl.graph) (void)cudaGraphExecDestroy(sl.graph);
+#endif
+}
+
 static void compositor_free(sb_compositor *c)
 {
     if (!c) return;
     cudaStream_t s = c->stream ? c->stream : default_stream();
-    if (c->stream) (void)cudaStreamSynchronize(c->stream);
-    for (auto p : c->src_dev) dev_free(p, s);
-    for (auto p : c->src4_dev) dev_free(p, s);
-    for (auto &v : c->src4_devx)
-        for (auto p : v) dev_free(p, s);
+    for (cudaStream_t q : {c->stream, c->h2d, c->d2h, c->comm_stream})  // nothing queued may still use what is freed
+        if (q) (void)cudaStreamSynchronize(q);
+    for (Slot &sl : c->slots) slot_free(sl, s);
     for (auto p : c->rgbm_dev) dev_free(p, s);
     for (auto p : c->tab_dev) dev_free(p, s);
     for (auto p : c->maps_dev) dev_free(p, s);
     for (auto p : c->usermask_dev) dev_free(p, s);
     for (auto &g : c->gain) gain_free(&g, s);
-    dev_free(c->out.rgb, s);
-    dev_free(c->out.mask, s);
     dev_free(c->flush_buf, s);
-    if (c->h2d) (void)cudaStreamSynchronize(c->h2d);
-    if (c->d2h) (void)cudaStreamSynchronize(c->d2h);
-    for (auto &v : c->src_devx)
-        for (auto p : v) dev_free(p, s);
-    if (c->pipe_ready) {
-        for (auto &o : c->outx) {
-            dev_free(o.rgb, s);
-            dev_free(o.mask, s);
-        }
-    }
-    for (int k = 0; k < SB_PIPE_DEPTH; ++k) {
-        if (c->e_h2d[k]) (void)cudaEventDestroy(c->e_h2d[k]);
-        if (c->e_comp[k]) (void)cudaEventDestroy(c->e_comp[k]);
-        if (c->e_d2h[k]) (void)cudaEventDestroy(c->e_d2h[k]);
-    }
     if (c->h2d) (void)cudaStreamDestroy(c->h2d);
     if (c->d2h) (void)cudaStreamDestroy(c->d2h);
-    if (c->comm_stream) {
-        (void)cudaStreamSynchronize(c->comm_stream);
-        (void)cudaStreamDestroy(c->comm_stream);
-    }
+    if (c->comm_stream) (void)cudaStreamDestroy(c->comm_stream);
     for (int k = 0; k < 2; ++k) {
         if (c->e_part[k]) (void)cudaEventDestroy(c->e_part[k]);
         if (c->e_xchg[k]) (void)cudaEventDestroy(c->e_xchg[k]);
     }
-#ifndef SB_EMU
-    for (auto &g : c->graph_exec)
-        if (g) (void)cudaGraphExecDestroy(g);
-#endif
     for (auto &e : c->tev) (void)cudaEventDestroy(e);
     c->shard.release(s);
     c->plan.release(s);
@@ -138,11 +149,6 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, int rank, int w
     c->count = n;
     if (c->sharded) ShardPlan::block_of(n, world, rank, &c->first, &c->count);
     auto mine = [&](int i) { return i >= c->first && i < c->first + c->count; };
-    c->warp_type = rig->warp_type;
-    c->scale = rig->scale;
-    c->blend_kind_requested = rig->blend_kind;
-    c->blend_strength = rig->blend_strength;
-    c->mask_mode = rig->mask_mode;
     SB_TRY(ensure_device());
     SB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     cudaStream_t s = c->stream;
@@ -151,8 +157,6 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, int rank, int w
     c->src_h.assign(rig->src_h, rig->src_h + n);
     c->rects.resize(n);
     c->jobs.resize(n);
-    c->src_dev.assign(n, nullptr);
-    c->src4_dev.assign(n, nullptr);
     {
         const char *e = getenv("SB_SRC4");  // SB_SRC4=0: the warp kernel reads the packed 3-byte sources (A/B switch)
         c->use_src4 = !(e && e[0] == '0');
@@ -181,7 +185,6 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, int rank, int w
         c->max_w = std::max(c->max_w, rect[2]);
         c->max_h = std::max(c->max_h, rect[3]);
         if (!mine(i)) continue;  // another rank warps this image: only its geometry is needed here
-        SB_TRY(dev_alloc((void **)&c->src_dev[i], (size_t)c->src_w[i] * 3 * c->src_h[i] + SB_SRC_PAD, s));
         SB_TRY(dev_alloc((void **)&c->rgbm_dev[i], (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
         // the row padding (never written by the warp kernel) is read by the tile kernels' 16-byte copies: weight 0
         SB_CUDA(cudaMemsetAsync(c->rgbm_dev[i], 0, (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
@@ -192,12 +195,7 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, int rank, int w
             SB_TRY(dev_alloc((void **)&c->maps_dev[i], (size_t)2 * rect[2] * rect[3] * sizeof(float), s));
             SB_TRY(warp_maps_upload(p, rect, c->maps_dev[i], &c->jobs[i], s));
         }
-        c->jobs[i].src = c->src_dev[i];
         c->jobs[i].spitch = (long long)c->src_w[i] * 3;
-        if (c->use_src4 && (long long)c->src_w[i] * c->src_h[i] < (1ll << 31)) {
-            SB_TRY(dev_alloc((void **)&c->src4_dev[i], ((size_t)c->src_w[i] * c->src_h[i] + 4) * sizeof(uint32_t), s));
-            c->jobs[i].src4 = c->src4_dev[i];
-        }
         c->jobs[i].dst_rgbm = c->rgbm_dev[i];
         c->jobs[i].rgbm_pitch = rgbm_pitch_of(rect[2]);
         c->warp_bytes += 3.0 * c->src_w[i] * c->src_h[i] + 4.0 * rect[2] * rect[3];
@@ -239,14 +237,57 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, int rank, int w
     }
     SB_TRY(c->plan.allocate(s));
     if (c->sharded) SB_TRY(c->shard.allocate(c->plan, s));
-    std::memset(&c->out, 0, sizeof c->out);
-    c->out.w = out_w;
-    c->out.h = out_h;
-    c->out.rgb_pitch = (long long)out_w * 3;
-    c->out.mask_pitch = out_w;
-    SB_TRY(dev_alloc((void **)&c->out.rgb, (size_t)std::max(out_w, 1) * 3 * std::max(out_h, 1), s));
-    SB_TRY(dev_alloc((void **)&c->out.mask, (size_t)std::max(out_w, 1) * std::max(out_h, 1), s));
+    c->slots[0].out.w = out_w;
+    c->slots[0].out.h = out_h;
+    SB_TRY(slot_alloc(c, c->slots[0]));
+    c->n_slots = 1;
+    for (int i = c->first; i < c->first + c->count; ++i) {
+        c->jobs[i].src = c->slots[0].src[i];
+        c->jobs[i].src4 = c->slots[0].src4[i];
+    }
     SB_CUDA(cudaStreamSynchronize(s));
+    return SB_OK;
+}
+
+// the jobs of `slot`: `jobs` with the slot's sources swapped in (built in a scratch vector: no allocation per step)
+static const WarpJob *slot_jobs_of(sb_compositor *c, int slot)
+{
+    if (slot == 0) return c->jobs.data();
+    c->slot_jobs = c->jobs;
+    for (int i = 0; i < c->n; ++i) {
+        c->slot_jobs[i].src = c->slots[slot].src[i];
+        c->slot_jobs[i].src4 = c->slots[slot].src4[i];
+    }
+    return c->slot_jobs.data();
+}
+
+// the jobs are baked into the captured steps: capture again on next use
+static void drop_graphs(sb_compositor *c)
+{
+#ifndef SB_EMU
+    for (Slot &sl : c->slots)
+        if (sl.graph) {
+            (void)cudaGraphExecDestroy(sl.graph);
+            sl.graph = nullptr;
+        }
+#endif
+}
+
+// image i blends with the mask in usermask_dev[i]: stored as its weight byte (and_validity 0) or ANDed with the
+// warped validity mask (1); the mask may hold gray values
+static void use_blend_mask(sb_compositor *c, int i, int and_validity)
+{
+    c->jobs[i].blend_mask = c->usermask_dev[i];
+    c->jobs[i].blend_mask_pitch = c->rects[i].w;
+    c->jobs[i].blend_mask_and = and_validity;
+    c->plan.binary_masks = false;
+    drop_graphs(c);
+}
+
+static int download_out(const PanoOut &o, uint8_t *dst, size_t dst_pitch, uint8_t *dst_mask, size_t mask_pitch, cudaStream_t s)
+{
+    if (dst) SB_CUDA(sb_copy2d(dst, dst_pitch, o.rgb, (size_t)o.rgb_pitch, (size_t)o.w * 3, o.h, cudaMemcpyDeviceToHost, s));
+    if (dst_mask) SB_CUDA(sb_copy2d(dst_mask, mask_pitch, o.mask, (size_t)o.mask_pitch, o.w, o.h, cudaMemcpyDeviceToHost, s));
     return SB_OK;
 }
 
@@ -263,7 +304,7 @@ static int compositor_enqueue(sb_compositor *c, bool events, int slot = 0)
     }();
     if (!events && use_graph && !c->sharded) {  // (the sharded step contains the NCCL exchange: launched directly)
         cudaStream_t s = c->stream;
-        if (!c->graph_exec[slot]) {
+        if (!c->slots[slot].graph) {
             const unsigned long long before = sb_launch_count();
             SB_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
             const int rc = compositor_enqueue_kernels(c, false, slot);
@@ -276,11 +317,11 @@ static int compositor_enqueue(sb_compositor *c, bool events, int slot = 0)
                 return rc;
             }
             if (e != cudaSuccess) return cuda_fail(e, "cudaStreamEndCapture", __FILE__, __LINE__);
-            const cudaError_t ei = cudaGraphInstantiate(&c->graph_exec[slot], g, 0);
+            const cudaError_t ei = cudaGraphInstantiate(&c->slots[slot].graph, g, 0);
             (void)cudaGraphDestroy(g);
             if (ei != cudaSuccess) return cuda_fail(ei, "cudaGraphInstantiate", __FILE__, __LINE__);
         }
-        SB_CUDA(cudaGraphLaunch(c->graph_exec[slot], s));
+        SB_CUDA(cudaGraphLaunch(c->slots[slot].graph, s));
         adjust_launch_count((long long)c->graph_kernels);
         return SB_OK;
     }
@@ -345,10 +386,9 @@ static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
         return SB_OK;
     };
     SB_TRY(mark("start"));
-    const WarpJob *jobs = slot ? c->jobsx[slot - 1].data() : c->jobs.data();
-    SB_TRY(launch_warp(jobs + c->first, c->count, s));
+    SB_TRY(launch_warp(slot_jobs_of(c, slot) + c->first, c->count, s));
     SB_TRY(mark("warp"));
-    const PanoOut &out = slot ? c->outx[slot - 1] : c->out;
+    const PanoOut &out = c->slots[slot].out;
     if (!c->sharded) return c->plan.run(out, s, events ? std::function<int(const std::string &)>(mark) : nullptr);
     if (!c->comm_stream) {
         SB_CUDA(cudaStreamCreateWithFlags(&c->comm_stream, cudaStreamNonBlocking));
@@ -462,74 +502,53 @@ static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
     return SB_OK;
 }
 
-// second buffer set + copy streams for sb_compositor_submit / _wait
+// the other slots and the copy streams of sb_compositor_submit / _wait, on the first submit
 static int compositor_pipe_init(sb_compositor *c)
 {
-    if (c->pipe_ready) return SB_OK;
-    cudaStream_t s = c->stream;
-    for (int k = 0; k < SB_PIPE_DEPTH - 1; ++k) {
-        c->src_devx[k].assign(c->n, nullptr);
-        c->jobsx[k] = c->jobs;
-        for (int i = 0; i < c->n; ++i) {
-            SB_TRY(dev_alloc((void **)&c->src_devx[k][i], (size_t)c->src_w[i] * 3 * c->src_h[i] + SB_SRC_PAD, s));
-            c->jobsx[k][i].src = c->src_devx[k][i];
-            if (c->jobs[i].src4) {
-                if (c->src4_devx[k].empty()) c->src4_devx[k].assign(c->n, nullptr);
-                SB_TRY(dev_alloc((void **)&c->src4_devx[k][i], ((size_t)c->src_w[i] * c->src_h[i] + 4) * sizeof(uint32_t), s));
-                c->jobsx[k][i].src4 = c->src4_devx[k][i];
-            }
-        }
-        c->outx[k] = c->out;
-        c->outx[k].rgb = nullptr;
-        c->outx[k].mask = nullptr;
-        SB_TRY(dev_alloc((void **)&c->outx[k].rgb, (size_t)c->out.w * 3 * c->out.h, s));
-        SB_TRY(dev_alloc((void **)&c->outx[k].mask, (size_t)c->out.w * c->out.h, s));
-    }
-    SB_CUDA(cudaStreamCreateWithFlags(&c->h2d, cudaStreamNonBlocking));
-    SB_CUDA(cudaStreamCreateWithFlags(&c->d2h, cudaStreamNonBlocking));
-    for (int k = 0; k < SB_PIPE_DEPTH; ++k) {
-        SB_CUDA(cudaEventCreateWithFlags(&c->e_h2d[k], cudaEventDisableTiming));
-        SB_CUDA(cudaEventCreateWithFlags(&c->e_comp[k], cudaEventDisableTiming));
-        SB_CUDA(cudaEventCreateWithFlags(&c->e_d2h[k], cudaEventDisableTiming));
-    }
-    SB_CUDA(cudaStreamSynchronize(s));
-    c->pipe_ready = true;
+    if (!c->h2d) SB_CUDA(cudaStreamCreateWithFlags(&c->h2d, cudaStreamNonBlocking));
+    if (!c->d2h) SB_CUDA(cudaStreamCreateWithFlags(&c->d2h, cudaStreamNonBlocking));
+    for (; c->n_slots < SB_PIPE_DEPTH; ++c->n_slots) SB_TRY(slot_alloc(c, c->slots[c->n_slots]));
+    SB_CUDA(cudaStreamSynchronize(c->stream));
     return SB_OK;
 }
 
-extern "C" {
-
-sb_compositor *sb_compositor_create(const sb_rig *rig)
+static bool valid_rig(const sb_rig *rig)
 {
-    if (!rig || rig->n_images <= 0 || rig->n_images > SB_MAX_IMAGES || !rig->src_w || !rig->src_h || !rig->K || !rig->R ||
-        rig->warp_type < SB_WARP_SPHERICAL || rig->warp_type > SB_WARP_TRANSVERSE_MERCATOR || rig->blend_kind < SB_BLEND_NO ||
-        rig->blend_kind > SB_BLEND_MULTIBAND) {
-        set_error("sb_compositor_create: invalid rig");
-        return nullptr;
-    }
-    sb_compositor *c = new sb_compositor;
-    if (compositor_build(c, rig, 0, 1) != SB_OK) {
-        compositor_free(c);
-        return nullptr;
-    }
-    return c;
+    return rig && rig->n_images > 0 && rig->n_images <= SB_MAX_IMAGES && rig->src_w && rig->src_h && rig->K && rig->R &&
+           rig->warp_type >= SB_WARP_SPHERICAL && rig->warp_type <= SB_WARP_TRANSVERSE_MERCATOR && rig->blend_kind >= SB_BLEND_NO &&
+           rig->blend_kind <= SB_BLEND_MULTIBAND;
 }
 
-// One panorama over `world` GPUs (one process each): this rank warps and pyramids images
-// [rank*n/world, (rank+1)*n/world) and owns one column strip of the panorama (sb_shard.h).
-sb_compositor *sb_compositor_create_sharded(const sb_rig *rig, int rank, int world)
+static sb_compositor *compositor_create(const sb_rig *rig, int rank, int world)
 {
-    if (!rig || rig->n_images <= 0 || rig->n_images > SB_MAX_IMAGES || !rig->src_w || !rig->src_h || !rig->K || !rig->R ||
-        rig->warp_type < SB_WARP_SPHERICAL || rig->warp_type > SB_WARP_TRANSVERSE_MERCATOR || world < 1 || rank < 0 || rank >= world) {
-        set_error("sb_compositor_create_sharded: invalid argument");
-        return nullptr;
-    }
     sb_compositor *c = new sb_compositor;
     if (compositor_build(c, rig, rank, world) != SB_OK) {
         compositor_free(c);
         return nullptr;
     }
     return c;
+}
+
+extern "C" {
+
+sb_compositor *sb_compositor_create(const sb_rig *rig)
+{
+    if (!valid_rig(rig)) {
+        set_error("sb_compositor_create: invalid rig");
+        return nullptr;
+    }
+    return compositor_create(rig, 0, 1);
+}
+
+// One panorama over `world` GPUs (one process each): this rank warps and pyramids images
+// [rank*n/world, (rank+1)*n/world) and owns one column strip of the panorama (sb_shard.h).
+sb_compositor *sb_compositor_create_sharded(const sb_rig *rig, int rank, int world)
+{
+    if (!valid_rig(rig) || world < 1 || rank < 0 || rank >= world) {
+        set_error("sb_compositor_create_sharded: invalid argument");
+        return nullptr;
+    }
+    return compositor_create(rig, rank, world);
 }
 
 int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_local, int strip[2])
@@ -562,9 +581,9 @@ int sb_compositor_shard_phase(sb_compositor *c, int phase)
         SB_TRY(launch_warp(c->jobs.data() + c->first, c->count, s));
         SB_TRY(shard_local(c, s, std::function<int(const std::string &)>(nomark)));
     } else if (c->plan.kind == SB_BLEND_FEATHER) {
-        SB_TRY(c->shard.feather_finish(c->plan, c->out, s));
+        SB_TRY(c->shard.feather_finish(c->plan, c->slots[0].out, s));
     } else {
-        SB_TRY(c->shard.finish(c->plan, c->out, s));
+        SB_TRY(c->shard.finish(c->plan, c->slots[0].out, s));
     }
     SB_CUDA(cudaStreamSynchronize(s));
     return SB_OK;
@@ -632,13 +651,14 @@ int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pit
         set_error("sb_compositor_upload: invalid argument");
         return SB_ERR_INVALID;
     }
-    if (!c->src_dev[i]) {
+    const Slot &sl = c->slots[0];
+    if (!sl.src[i]) {
         set_error("sb_compositor_upload: image %d belongs to another rank (this rank owns %d..%d)", i, c->first, c->first + c->count - 1);
         return SB_ERR_INVALID;
     }
-    SB_CUDA(sb_copy2d(c->src_dev[i], (size_t)c->src_w[i] * 3, src, pitch, (size_t)c->src_w[i] * 3, c->src_h[i],
+    SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->src_w[i] * 3, src, pitch, (size_t)c->src_w[i] * 3, c->src_h[i],
                               cudaMemcpyHostToDevice, c->stream));
-    if (c->src4_dev[i]) SB_TRY(launch_repack_rgbx(c->src_dev[i], c->src4_dev[i], (long long)c->src_w[i] * c->src_h[i], c->stream));
+    if (sl.src4[i]) SB_TRY(launch_repack_rgbx(sl.src[i], sl.src4[i], (long long)c->src_w[i] * c->src_h[i], c->stream));
     if (!pinned) SB_CUDA(cudaStreamSynchronize(c->stream));
     return SB_OK;
 }
@@ -655,23 +675,7 @@ int sb_compositor_set_mask(sb_compositor *c, int i, const uint8_t *mask, size_t 
     if (!c->usermask_dev[i]) SB_TRY(dev_alloc((void **)&c->usermask_dev[i], (size_t)w * h, c->stream));
     SB_CUDA(sb_copy2d(c->usermask_dev[i], w, mask, pitch, w, h, cudaMemcpyHostToDevice, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
-    c->jobs[i].blend_mask = c->usermask_dev[i];
-    c->jobs[i].blend_mask_pitch = w;
-    c->jobs[i].blend_mask_and = 0;
-    c->plan.binary_masks = false;  // a caller's mask may hold gray values
-    for (auto &jx : c->jobsx)
-        if (!jx.empty()) {
-            jx[i].blend_mask = c->usermask_dev[i];
-            jx[i].blend_mask_pitch = w;
-            jx[i].blend_mask_and = 0;
-        }
-#ifndef SB_EMU
-    for (auto &g : c->graph_exec)  // the jobs are baked into the captured launches: re-capture
-        if (g) {
-            (void)cudaGraphExecDestroy(g);
-            g = nullptr;
-        }
-#endif
+    use_blend_mask(c, i, 0);
     return SB_OK;
 }
 
@@ -687,23 +691,7 @@ int sb_compositor_set_seam_mask(sb_compositor *c, int i, const uint8_t *seam, si
     const int w = c->rects[i].w, h = c->rects[i].h;
     if (!c->usermask_dev[i]) SB_TRY(dev_alloc((void **)&c->usermask_dev[i], (size_t)w * h, c->stream));
     SB_TRY(seam_resize_device(seam, seam_pitch, sw, sh, nullptr, 0, c->usermask_dev[i], w, w, h, c->stream));
-    c->jobs[i].blend_mask = c->usermask_dev[i];
-    c->jobs[i].blend_mask_pitch = w;
-    c->jobs[i].blend_mask_and = 1;
-    c->plan.binary_masks = false;  // the resized seam mask is bilinear: gray along the seam
-    for (auto &jx : c->jobsx)
-        if (!jx.empty()) {
-            jx[i].blend_mask = c->usermask_dev[i];
-            jx[i].blend_mask_pitch = w;
-            jx[i].blend_mask_and = 1;
-        }
-#ifndef SB_EMU
-    for (auto &g : c->graph_exec)  // the jobs are baked into the captured launches: re-capture
-        if (g) {
-            (void)cudaGraphExecDestroy(g);
-            g = nullptr;
-        }
-#endif
+    use_blend_mask(c, i, 1);
     return SB_OK;
 }
 
@@ -717,30 +705,8 @@ int sb_compositor_set_gain(sb_compositor *c, int i, const float *gain_map, int g
     // ExposureErrorCompensator.apply(i, corner, warped image, mask) (exposure_error_compensator.py:43-45,
     // stitcher.py:219-221) fused into the warp's epilogue: the warped image never exists uncompensated
     SB_CUDA(cudaStreamSynchronize(c->stream));  // the previous run may still read the old gain buffers
-    WarpJob fields = c->jobs[i];
-    SB_TRY(gain_upload(&fields, &c->gain[i], c->rects[i].w, c->rects[i].h, gain_map, gw, gh, gc, gain_scalar, c->stream));
-    auto copy_gain = [&](WarpJob &j) {
-        j.gain_mode = fields.gain_mode;
-        j.gain_gw = fields.gain_gw;
-        j.gain_gc = fields.gain_gc;
-        j.gain_map = fields.gain_map;
-        j.gain_tx = fields.gain_tx;
-        j.gain_ty = fields.gain_ty;
-        j.gain_fx = fields.gain_fx;
-        j.gain_fy = fields.gain_fy;
-        j.gain_lut = fields.gain_lut;
-    };
-    copy_gain(c->jobs[i]);
-    for (auto &jx : c->jobsx)
-        if (!jx.empty()) copy_gain(jx[i]);
-#ifndef SB_EMU
-    for (auto &g : c->graph_exec)  // the jobs are baked into the captured launches: re-capture
-        if (g) {
-            (void)cudaGraphExecDestroy(g);
-            g = nullptr;
-        }
-#endif
-    return SB_OK;
+    drop_graphs(c);  // before the upload, which frees the buffers they read
+    return gain_upload(&c->jobs[i], &c->gain[i], c->rects[i].w, c->rects[i].h, gain_map, gw, gh, gc, gain_scalar, c->stream);
 }
 
 int sb_compositor_run(sb_compositor *c)
@@ -761,16 +727,11 @@ int sb_compositor_sync(sb_compositor *c)
 
 int sb_compositor_download(sb_compositor *c, uint8_t *dst, size_t dst_pitch, uint8_t *dst_mask, size_t mask_pitch)
 {
-    if (!c || (dst && dst_pitch < (size_t)c->out.w * 3) || (dst_mask && mask_pitch < (size_t)c->out.w)) {
+    if (!c || (dst && dst_pitch < (size_t)c->slots[0].out.w * 3) || (dst_mask && mask_pitch < (size_t)c->slots[0].out.w)) {
         set_error("sb_compositor_download: invalid argument");
         return SB_ERR_INVALID;
     }
-    if (dst)
-        SB_CUDA(sb_copy2d(dst, dst_pitch, c->out.rgb, (size_t)c->out.rgb_pitch, (size_t)c->out.w * 3, c->out.h,
-                                  cudaMemcpyDeviceToHost, c->stream));
-    if (dst_mask)
-        SB_CUDA(sb_copy2d(dst_mask, mask_pitch, c->out.mask, (size_t)c->out.mask_pitch, c->out.w, c->out.h,
-                                  cudaMemcpyDeviceToHost, c->stream));
+    SB_TRY(download_out(c->slots[0].out, dst, dst_pitch, dst_mask, mask_pitch, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
     return SB_OK;
 }
@@ -780,7 +741,7 @@ int sb_compositor_download(sb_compositor *c, uint8_t *dst, size_t dst_pitch, uin
 int sb_compositor_submit(sb_compositor *c, const uint8_t *const *srcs, const size_t *pitches, uint8_t *dst, size_t dst_pitch,
                          uint8_t *dst_mask, size_t mask_pitch, unsigned long long *ticket)
 {
-    if (!c || !srcs || !pitches || (dst && dst_pitch < (size_t)c->out.w * 3) || (dst_mask && mask_pitch < (size_t)c->out.w)) {
+    if (!c || !srcs || !pitches || (dst && dst_pitch < (size_t)c->slots[0].out.w * 3) || (dst_mask && mask_pitch < (size_t)c->slots[0].out.w)) {
         set_error("sb_compositor_submit: invalid argument");
         return SB_ERR_INVALID;
     }
@@ -793,37 +754,31 @@ int sb_compositor_submit(sb_compositor *c, const uint8_t *const *srcs, const siz
             set_error("sb_compositor_submit: invalid source %d", i);
             return SB_ERR_INVALID;
         }
-    SB_TRY(compositor_pipe_init(c));
+    if (c->n_slots < SB_PIPE_DEPTH) SB_TRY(compositor_pipe_init(c));
     const unsigned long long t = c->submitted;
     const int slot = (int)(t % SB_PIPE_DEPTH);
-    const std::vector<uint8_t *> &sdev = slot ? c->src_devx[slot - 1] : c->src_dev;
-    const PanoOut &o = slot ? c->outx[slot - 1] : c->out;
+    Slot &sl = c->slots[slot];
     // sources of this slot are free once the previous compute that read them has finished; on a slot's first use
     // that is whatever upload() / run() / sb_compositor_time() queued on the compute stream before this submit
     // (download() is synchronous, so the output buffers need no such guard)
-    if (t < SB_PIPE_DEPTH) SB_CUDA(cudaEventRecord(c->e_comp[slot], c->stream));
-    SB_CUDA(cudaStreamWaitEvent(c->h2d, c->e_comp[slot], 0));
+    if (t < SB_PIPE_DEPTH) SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
+    SB_CUDA(cudaStreamWaitEvent(c->h2d, sl.e_comp, 0));
     for (int i = 0; i < c->n; ++i)
-        SB_CUDA(sb_copy2d(sdev[i], (size_t)c->src_w[i] * 3, srcs[i], pitches[i], (size_t)c->src_w[i] * 3, c->src_h[i],
+        SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->src_w[i] * 3, srcs[i], pitches[i], (size_t)c->src_w[i] * 3, c->src_h[i],
                                   cudaMemcpyHostToDevice, c->h2d));
     // the repack kernels follow the LAST copy (same stream): a kernel between two copies would leave the PCIe link idle
     // for its launch + run time, eight times per step
-    for (int i = 0; i < c->n; ++i) {
-        uint32_t *s4 = slot ? (c->src4_devx[slot - 1].empty() ? nullptr : c->src4_devx[slot - 1][i]) : c->src4_dev[i];
-        if (s4) SB_TRY(launch_repack_rgbx(sdev[i], s4, (long long)c->src_w[i] * c->src_h[i], c->h2d));
-    }
-    SB_CUDA(cudaEventRecord(c->e_h2d[slot], c->h2d));
-    SB_CUDA(cudaStreamWaitEvent(c->stream, c->e_h2d[slot], 0));
+    for (int i = 0; i < c->n; ++i)
+        if (sl.src4[i]) SB_TRY(launch_repack_rgbx(sl.src[i], sl.src4[i], (long long)c->src_w[i] * c->src_h[i], c->h2d));
+    SB_CUDA(cudaEventRecord(sl.e_h2d, c->h2d));
+    SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_h2d, 0));
     // the output buffers of this slot are free once their previous download has finished
-    if (t >= SB_PIPE_DEPTH) SB_CUDA(cudaStreamWaitEvent(c->stream, c->e_d2h[slot], 0));
+    if (t >= SB_PIPE_DEPTH) SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_d2h, 0));
     SB_TRY(compositor_enqueue(c, false, slot));
-    SB_CUDA(cudaEventRecord(c->e_comp[slot], c->stream));
-    SB_CUDA(cudaStreamWaitEvent(c->d2h, c->e_comp[slot], 0));
-    if (dst)
-        SB_CUDA(sb_copy2d(dst, dst_pitch, o.rgb, (size_t)o.rgb_pitch, (size_t)o.w * 3, o.h, cudaMemcpyDeviceToHost, c->d2h));
-    if (dst_mask)
-        SB_CUDA(sb_copy2d(dst_mask, mask_pitch, o.mask, (size_t)o.mask_pitch, o.w, o.h, cudaMemcpyDeviceToHost, c->d2h));
-    SB_CUDA(cudaEventRecord(c->e_d2h[slot], c->d2h));
+    SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
+    SB_CUDA(cudaStreamWaitEvent(c->d2h, sl.e_comp, 0));
+    SB_TRY(download_out(sl.out, dst, dst_pitch, dst_mask, mask_pitch, c->d2h));
+    SB_CUDA(cudaEventRecord(sl.e_d2h, c->d2h));
     c->submitted = t + 1;
     if (ticket) *ticket = t;
     return SB_OK;
@@ -831,11 +786,11 @@ int sb_compositor_submit(sb_compositor *c, const uint8_t *const *srcs, const siz
 
 int sb_compositor_wait(sb_compositor *c, unsigned long long ticket)
 {
-    if (!c || !c->pipe_ready || ticket >= c->submitted || ticket + SB_PIPE_DEPTH < c->submitted) {
+    if (!c || c->n_slots < SB_PIPE_DEPTH || ticket >= c->submitted || ticket + SB_PIPE_DEPTH < c->submitted) {
         set_error("sb_compositor_wait: ticket %llu is not in flight", ticket);
         return SB_ERR_STATE;
     }
-    SB_CUDA(cudaEventSynchronize(c->e_d2h[ticket % SB_PIPE_DEPTH]));
+    SB_CUDA(cudaEventSynchronize(c->slots[ticket % SB_PIPE_DEPTH].e_d2h));
     return SB_OK;
 }
 

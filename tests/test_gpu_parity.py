@@ -288,6 +288,12 @@ def test_pipelined_submit_wait(cuda_lib):
     c.close()
 
 
+def test_setters_between_pipelined_submits(cuda_lib):
+    import test_host_logic
+
+    test_host_logic.check_setters_between_submits(4)
+
+
 def test_simple_and_fast_kernels_agree(cuda_lib):
     """A/B inside one process is not possible (the variant is chosen once per process): run the other variant in
     a child process and compare panoramas byte for byte."""

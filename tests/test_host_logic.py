@@ -166,6 +166,49 @@ def test_pipelined_submit_wait_equals_composite(use_emu):
     c.close()
 
 
+def check_setters_between_submits(scale_down):
+    """set_mask, set_gain and set_seam_mask between pipelined submits reach every buffer slot: each result equals
+    composite() of the same batch on a second compositor given the same settings.  Three submits before and after the
+    settings use every slot (on the GPU: capture its step, then drop and capture it again)."""
+    cfg = rigs.config("cfg2", scale_down)
+    cams = cfg["cameras"]
+    args = (cams, [(cfg["w"], cfg["h"])] * len(cams), cfg["warper"], cfg["blender"], cfg["strength"])
+    c, ref = Compositor(*args), Compositor(*args)
+    _, _, pw, ph = c.roi
+    outs = [(c.pinned_empty((ph, pw, 3)), c.pinned_empty((ph, pw))) for _ in range(3)]
+
+    def three_steps(b0):
+        batches = []
+        for b in range(b0, b0 + 3):
+            pinned = [c.pinned_empty((cfg["h"], cfg["w"], 3)) for _ in cams]
+            for i, p in enumerate(pinned):
+                p[...] = rigs.noise_image(cfg["h"], cfg["w"], 10 * b + i)
+            batches.append(pinned)
+        tickets = [c.submit(b, *o) for b, o in zip(batches, outs)]
+        for k, (b, t, o) in enumerate(zip(batches, tickets, outs)):
+            c.wait(t)
+            pano, mask = ref.composite(b)
+            assert np.array_equal(o[0], pano) and np.array_equal(o[1], mask), f"batch {b0 + k}"
+
+    three_steps(0)
+    _, _, w1, h1 = c.rects[1]
+    ramp = np.tile(np.linspace(0, 255, w1).astype(np.uint8), (h1, 1))
+    gain = np.linspace(0.7, 1.3, 12, dtype=np.float32).reshape(3, 4)
+    _, _, w5, h5 = c.rects[5]
+    seam = np.where(np.random.default_rng(5).random((h5 // 4, w5 // 4)) < 0.7, 255, 0).astype(np.uint8)  # low resolution
+    for x in (c, ref):
+        x.set_mask(1, ramp)
+        x.set_gain(3, gain)
+        x.set_seam_mask(5, seam)
+    three_steps(3)
+    c.close()
+    ref.close()
+
+
+def test_setters_between_pipelined_submits(use_emu):
+    check_setters_between_submits(25)
+
+
 def test_band_clipping_matches_oracle(use_emu, oracle):
     """MultiBandBlender::prepare's band clipping -- product plan vs oracle restatement."""
     rng = np.random.default_rng(3)

@@ -112,6 +112,27 @@ def test_sharded_rejects_what_it_cannot_do(use_emu):
     c.close()
 
 
+def test_sharded_create_rejects_an_unknown_blend_kind(use_emu):
+    """Both creates check the rig alike: a blend kind outside sb_blend_kind is refused, not built as a feather blend."""
+    from stitching_b200 import Warper, _lib
+
+    cams = rigs.yaw_ring(4, 64, 48, 70, 25)  # blocks run left to right: a feather blend of this rig can be sharded
+    K = np.ascontiguousarray(np.stack([Warper.get_K(cam, 1) for cam in cams]).astype(np.float32))
+    R = np.ascontiguousarray(np.stack([cam.R for cam in cams]).astype(np.float32))
+    w, h = (C.c_int * 4)(*[64] * 4), (C.c_int * 4)(*[48] * 4)
+
+    def create_sharded(kind):
+        rig = _lib.Rig(4, _lib.WARP_TYPES["spherical"], 70.0, kind, 5.0, w, h, K.ctypes.data_as(_lib.c_float_p),
+                       R.ctypes.data_as(_lib.c_float_p), 0)
+        return use_emu.sb_compositor_create_sharded(C.byref(rig), 0, 2)
+
+    c = create_sharded(_lib.BLEND_KINDS["feather"])
+    assert c
+    use_emu.sb_compositor_destroy(c)
+    assert not create_sharded(7)
+    assert b"invalid" in use_emu.sb_last_error()
+
+
 GLOO_WORKER = r"""
 import os, sys
 sys.path.insert(0, sys.argv[1])
