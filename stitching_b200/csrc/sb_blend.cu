@@ -229,7 +229,7 @@ int launch_collapse(const FeedImage *imgs_dev, const FeedImage *imgs_host, const
 {
     int gw = l == 0 ? out.w : lw, gh = l == 0 ? out.h : lh;
     if (gw <= 0 || gh <= 0) return SB_OK;
-    // the fast kernel works on byte-fed images (RGBM level 0, lane-pair levels) and needs at least one band
+    // the fast kernel works on byte-fed images (RGBM level 0, one colour word per pixel above) and needs at least one band
     bool packed = true;
     for (int i = 0; i < n; ++i) packed = packed && imgs_host[i].rgbm != nullptr;
     if (!use_simple_kernels() && nb >= 1 && packed) {

@@ -5,9 +5,9 @@
 // profile showed the kernel to be issue-bound rather than HBM-bound:
 //   * one thread per 2x2 quad: the four pixels share the 3x3 neighbourhood of the coarser level, so each pyrUp
 //     (of the image's G_{l+1} and of the collapsed C_{l+1}) is 9 taps per quad, evaluated through shared column sums;
-//   * the fed images' levels are byte-valued LANE PAIRS (sb_internal.h): red and blue run as two 16-bit lanes of
-//     one word through the pyrUp, the Laplacian and the accumulators (lane-wise VIADD.16x2 = the wrap-around of a
-//     short), a tap is one 8-byte load;
+//   * the fed images' levels are one word of bytes per pixel (sb_internal.h), a tap is one 4-byte load: split into
+//     lanes after the load, red and blue run as two 16-bit lanes of one word through the pyrUp, the Laplacian and the
+//     accumulators (lane-wise VIADD.16x2 = the wrap-around of a short);
 //   * compact 16-byte-aligned descriptors (ColDesc) read with vector loads, 32-bit element offsets;
 //   * exact early-outs: a fed image whose four weights in the quad are all zero contributes
 //     (short)trunc(L * 0) = 0 and wsum + 0 = wsum, i.e. nothing -- at level 0 this is the whole padding ring
@@ -69,20 +69,25 @@ __device__ __forceinline__ unsigned lanes(int lo, int hi) { return ((unsigned)lo
 __device__ __forceinline__ int lane_lo(unsigned v) { return (int)(short)(v & 0xffffu); }
 __device__ __forceinline__ int lane_hi(unsigned v) { return (int)v >> 16; }
 
-// The same pyrUp for a fed image's level stored as lane pairs (x = r | b << 16, y = g; all bytes): red and blue go
-// through the column sums and the final sums as two lanes of one word -- the largest intermediate, 64 * 255 + 32,
-// stays below 2^15, so the lanes never meet.  Results: u_rb = r | b << 16, u_g = g, each 0..255.
-__device__ __forceinline__ void up_quad_lanes(const uint2 *__restrict__ S, const Nbr &q, unsigned u_rb[2][2], unsigned u_g[2][2])
+// split a colour word r | g << 8 | b << 16 (byte 3 zero) into the lanes r | b << 16 and g
+__device__ __forceinline__ unsigned word_rb(unsigned v) { return v & 0x00ff00ffu; }
+__device__ __forceinline__ unsigned word_g(unsigned v) { return __byte_perm(v, 0u, 0x4441); }
+
+// The same pyrUp for a fed image's level stored as one word per pixel (r | g << 8 | b << 16): every tap is split into
+// the lanes r | b << 16 and g, and red and blue go through the column sums and the final sums as two lanes of one
+// word -- the largest intermediate, 64 * 255 + 32, stays below 2^15, so the lanes never meet.  Results:
+// u_rb = r | b << 16, u_g = g, each 0..255.
+__device__ __forceinline__ void up_quad_lanes(const uint32_t *__restrict__ S, const Nbr &q, unsigned u_rb[2][2], unsigned u_g[2][2])
 {
     unsigned e_rb[3], o_rb[3], e_g[3], o_g[3];
     const int cols[3] = {q.xp, q.xc, q.xn};
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-        const uint2 a0 = __ldg(S + q.rp + cols[k]), a1 = __ldg(S + q.rc + cols[k]), a2 = __ldg(S + q.rn + cols[k]);
-        e_rb[k] = a0.x + a2.x + 6u * a1.x;
-        o_rb[k] = a1.x + a2.x;
-        e_g[k] = a0.y + a2.y + 6u * a1.y;
-        o_g[k] = a1.y + a2.y;
+        const unsigned a0 = __ldg(S + q.rp + cols[k]), a1 = __ldg(S + q.rc + cols[k]), a2 = __ldg(S + q.rn + cols[k]);
+        e_rb[k] = word_rb(a0) + word_rb(a2) + 6u * word_rb(a1);
+        o_rb[k] = word_rb(a1) + word_rb(a2);
+        e_g[k] = word_g(a0) + word_g(a2) + 6u * word_g(a1);
+        o_g[k] = word_g(a1) + word_g(a2);
     }
     const unsigned M = 0x00ff00ffu;
     u_rb[0][0] = ((e_rb[0] + e_rb[2] + 6u * e_rb[1] + 0x00200020u) >> 6) & M;
@@ -218,15 +223,21 @@ __global__ void __launch_bounds__(CF_BX *CF_BY, 5) k_collapse_fast(const __grid_
                     wt[dy][dx] = fmul((float)(p[dy][dx] >> 24), SB_INV255);
                 }
         } else if (LV == 1) {
-            const int o0 = Y * s1.y + X;  // X even: the pairs are 8- / 16-byte aligned
+            const int o0 = Y * s1.y + X;  // X even: the pairs are 8-byte aligned
             const float2 w0 = __ldg(reinterpret_cast<const float2 *>(d.w + o0));
             const float2 w1 = __ldg(reinterpret_cast<const float2 *>(d.w + o0 + s1.y));
             if (w0.x == 0.f && w0.y == 0.f && w1.x == 0.f && w1.y == 0.f) continue;  // contributes exactly nothing
             wt[0][0] = w0.x; wt[0][1] = w0.y; wt[1][0] = w1.x; wt[1][1] = w1.y;
-            const uint4 a = __ldg(reinterpret_cast<const uint4 *>(d.q + o0));
-            const uint4 b = __ldg(reinterpret_cast<const uint4 *>(d.q + o0 + s1.y));
-            g_rb[0][0] = a.x; g_g[0][0] = a.y; g_rb[0][1] = a.z; g_g[0][1] = a.w;
-            g_rb[1][0] = b.x; g_g[1][0] = b.y; g_rb[1][1] = b.z; g_g[1][1] = b.w;
+            const uint2 a = __ldg(reinterpret_cast<const uint2 *>(d.q + o0));
+            const uint2 b = __ldg(reinterpret_cast<const uint2 *>(d.q + o0 + s1.y));
+            const unsigned p[2][2] = {{a.x, a.y}, {b.x, b.y}};
+#pragma unroll
+            for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+                for (int dx = 0; dx < 2; ++dx) {
+                    g_rb[dy][dx] = word_rb(p[dy][dx]);
+                    g_g[dy][dx] = word_g(p[dy][dx]);
+                }
         } else {
 #pragma unroll
             for (int dy = 0; dy < 2; ++dy)
@@ -237,9 +248,9 @@ __global__ void __launch_bounds__(CF_BX *CF_BY, 5) k_collapse_fast(const __grid_
                     if (!in[dy][dx]) continue;
                     const int o = (Y + dy) * s1.y + X + dx;
                     wt[dy][dx] = d.w[o];
-                    const uint2 v = __ldg(d.q + o);
-                    g_rb[dy][dx] = v.x;
-                    g_g[dy][dx] = v.y;
+                    const unsigned v = __ldg(d.q + o);
+                    g_rb[dy][dx] = word_rb(v);
+                    g_g[dy][dx] = word_g(v);
                 }
         }
         // Laplacian = level - pyrUp(next level); both are bytes, the difference fits a signed 16-bit lane (and the

@@ -11,7 +11,7 @@
 // Here a CTA owns a 64x16 tile (one thread per 2x2 quad) and stages every window the tile needs in shared memory with
 // asynchronous 16-byte copies (cp.async / LDGSTS, zero fill outside the source, the next image's windows in flight
 // while the current one is consumed): per covering image the 64x16 level-l pixels (level 0: packed RGBM; above: colour
-// lane pairs + weights) and the 34x10 window of level l+1 that holds the 3x3 pyrUp neighbourhoods of all quads, plus
+// words + weights) and the 34x10 window of level l+1 that holds the 3x3 pyrUp neighbourhoods of all quads, plus
 // the 34x10x3 window of the collapsed level C_{l+1}.  Elements outside a source arrive as zeros, which is exactly
 // "weight 0": no rect tests and no predicated taps in the consumers, whose shared-memory loads sit at compile-time
 // offsets.  The pyrUp is separable and neighbouring quads share two of their three coarse columns: every thread
@@ -48,10 +48,11 @@ constexpr int UPW = SB_TILE_UPW, UPH = SB_TILE_UPH;
 // Window geometry.  A staged row starts at a 16-byte boundary of its source row, so the logical window sits at a small
 // column offset inside the staged one: the window of the collapsed level (origin = 32 k - 1 int16 elements) at +7; the
 // windows of an image at offsets that depend on where its rect starts on the pano lattice (tile-uniform, run time):
-// RGBM and weights at (tile_x - rect_x) & 3 elements, the 8-byte lane pairs of the coarser level at origin & 1.
-constexpr int UPS = UPW + 2;                 // staged lane-pair window: 36 columns = 18 chunks, logical origin at +0 / +1 (run time)
+// RGBM, colour words and weights at (tile_x - rect_x) & 3 elements (0 or 2 above level 0, where rect origins are even),
+// the colour words of the coarser level at origin & 3.
+constexpr int UPS = 40;                      // staged coarse window: 40 words = 10 chunks, logical origin at +0 .. +3 (run time)
 constexpr int C1S = 48, C1O = 7;             // staged int16 window: 48 columns = 6 chunks
-constexpr int RGS = TW + 4;                  // staged RGBM window: 68 pixels = 17 chunks
+constexpr int RGS = TW + 4;                  // staged level-l window: 68 pixels = 17 chunks
 
 // the staged windows of one covering image
 template <int LV>
@@ -59,13 +60,13 @@ struct ItemBuf;
 template <>
 struct alignas(16) ItemBuf<0> {
     uint32_t own[TH][RGS];  // packed RGBM, zero outside the image
-    uint2 up[UPH][UPS];     // level-1 lane pairs around the tile
+    uint32_t up[UPH][UPS];  // level-1 colour words around the tile
 };
 template <>
 struct alignas(16) ItemBuf<1> {
-    uint2 own[TH][TW];      // level-l lane pairs (rect origins are even: 16-byte rows)
+    uint32_t own[TH][RGS];  // level-l colour words
     float w[TH][RGS];       // level-l weights, zero outside the padded rect
-    uint2 up[UPH][UPS];
+    uint32_t up[UPH][UPS];
 };
 
 template <int LV>
@@ -131,16 +132,19 @@ __device__ __forceinline__ void fix_borders(T (*t)[STRIDE], int bx, int by, int 
     __syncthreads();
 }
 
-// vertical column sums of coarse column `col` for the quads of row `row` (lane pairs: two 16-bit lanes per word; the
-// largest value, 8 * 255, leaves room for the horizontal pass: 8 * 2040 + 32 < 2^15)
-__device__ __forceinline__ void colsum_lanes(const uint2 (*up)[UPS], uint4 (*cs)[UPW], int col, int row)  // col: staged column
+// vertical column sums of coarse column `col` for the quads of row `row`: each colour word is split into the lanes
+// r | b << 16 and g (two 16-bit lanes per word; the largest value, 8 * 255, leaves room for the horizontal pass:
+// 8 * 2040 + 32 < 2^15)
+__device__ __forceinline__ void colsum_lanes(const uint32_t (*up)[UPS], uint4 (*cs)[UPW], int col, int row)  // col: logical column
 {
-    const uint2 a0 = up[row][col], a1 = up[row + 1][col], a2 = up[row + 2][col];
+    const unsigned a0 = up[row][col], a1 = up[row + 1][col], a2 = up[row + 2][col];
+    const unsigned M = 0x00ff00ffu;
+    const unsigned g0 = __byte_perm(a0, 0u, 0x4441), g1 = __byte_perm(a1, 0u, 0x4441), g2 = __byte_perm(a2, 0u, 0x4441);
     uint4 v;
-    v.x = a0.x + a2.x + 6u * a1.x;  // even output row: 1 6 1
-    v.y = a1.x + a2.x;              // odd output row: 4 4 (the factor lives in the final shift)
-    v.z = a0.y + a2.y + 6u * a1.y;
-    v.w = a1.y + a2.y;
+    v.x = (a0 & M) + (a2 & M) + 6u * (a1 & M);  // even output row: 1 6 1
+    v.y = (a1 & M) + (a2 & M);                  // odd output row: 4 4 (the factor lives in the final shift)
+    v.z = g0 + g2 + 6u * g1;
+    v.w = g1 + g2;
     cs[row][col] = v;
 }
 
@@ -169,8 +173,10 @@ __device__ __forceinline__ unsigned norm_two2(unsigned a)
     return __vadd2((xb >> 1) & 0x7fff7fffu, 0xfe00fe00u);                                   // - 512 per lane
 }
 
+// resident CTAs per SM: level 0 (24 KB of shared memory) 6; level 1 (33 KB with one colour word per pixel) 5 -- 48
+// registers, no spills (6 would spill)
 template <int LV, bool SLABS>
-__global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 4) k_collapse_tile(const __grid_constant__ CollapseArgs A)
+__global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 5) k_collapse_tile(const __grid_constant__ CollapseArgs A)
 {
     grid_dependency_sync();
 #ifndef SB_EMU
@@ -239,25 +245,21 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 4) k_collapse_tile(const
             }
         } else {
             const int X = tile_x - o.x, row = tile_y - o.y + 2 * ty;  // X even (rect origins below the top level are even)
-            {
-                const unsigned pb = 8u * (unsigned)cd.pitch;
-                const int xb = 8 * X + 16 * tx, rb = (8 * r.z + 15) & ~15;
-                stage_chunk(&B.own[2 * ty][2 * tx], cd.q, pb, row, r.w, xb, rb);
-                stage_chunk(&B.own[2 * ty + 1][2 * tx], cd.q, pb, row + 1, r.w, xb, rb);
-            }
-            if (tx < RGS / 4) {
+            if (tx < RGS / 4) {  // colours and weights: same element size, same chunks
                 const unsigned pb = 4u * (unsigned)cd.pitch;
                 const int xb = 4 * (X & ~3) + 16 * tx, rb = (4 * r.z + 15) & ~15;
+                stage_chunk(&B.own[2 * ty][4 * tx], cd.q, pb, row, r.w, xb, rb);
+                stage_chunk(&B.own[2 * ty + 1][4 * tx], cd.q, pb, row + 1, r.w, xb, rb);
                 stage_chunk(&B.w[2 * ty][4 * tx], cd.w, pb, row, r.w, xb, rb);
                 stage_chunk(&B.w[2 * ty + 1][4 * tx], cd.w, pb, row + 1, r.w, xb, rb);
             }
         }
-        if (tx < UPS / 2) {
-            const int bx = (((tile_x - o.x) >> 1) - 1) & ~1, by = ((tile_y - o.y) >> 1) - 1;  // the even column at or left of the origin
-            const unsigned pb = 8u * (unsigned)cd.upitch;
-            const int xb = 8 * bx + 16 * tx, rb = (8 * o.z + 15) & ~15;
-            stage_chunk(&B.up[ty][2 * tx], cd.uq, pb, by + ty, o.w, xb, rb);
-            if (ty < UPH - QY) stage_chunk(&B.up[QY + ty][2 * tx], cd.uq, pb, by + QY + ty, o.w, xb, rb);
+        if (tx < UPS / 4) {
+            const int bx = (((tile_x - o.x) >> 1) - 1) & ~3, by = ((tile_y - o.y) >> 1) - 1;  // the multiple of 4 at or left of the origin
+            const unsigned pb = 4u * (unsigned)cd.upitch;
+            const int xb = 4 * bx + 16 * tx, rb = (4 * o.z + 15) & ~15;
+            stage_chunk(&B.up[ty][4 * tx], cd.uq, pb, by + ty, o.w, xb, rb);
+            if (ty < UPH - QY) stage_chunk(&B.up[QY + ty][4 * tx], cd.uq, pb, by + QY + ty, o.w, xb, rb);
         }
         cp_async_commit();
     };
@@ -303,12 +305,12 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 4) k_collapse_tile(const
         }
         const int4 o = __ldg(reinterpret_cast<const int4 *>(&d.ox));  // ox, oy, uw, uh
         const int bx = ((tile_x - o.x) >> 1) - 1, by = ((tile_y - o.y) >> 1) - 1;
-        const int su = bx & 1;  // logical column c of the coarse window = staged column c + su
+        const int su = bx & 3;  // logical column c of the coarse window = staged column c + su
         if (bx < 0 || by < 0 || bx + UPW > o.z || by + UPH > o.w)
-            fix_borders<uint2, UPH, UPW, UPS>(reinterpret_cast<uint2(*)[UPS]>(&B.up[0][su]), bx, by, o.z, o.w, tid);
+            fix_borders<uint32_t, UPH, UPW, UPS>(reinterpret_cast<uint32_t(*)[UPS]>(&B.up[0][su]), bx, by, o.z, o.w, tid);
         uint4(*cs)[UPW] = S.cs[k & 1];
         {
-            const uint2(*ups)[UPS] = reinterpret_cast<const uint2(*)[UPS]>(&B.up[0][su]);
+            const uint32_t(*ups)[UPS] = reinterpret_cast<const uint32_t(*)[UPS]>(&B.up[0][su]);
             colsum_lanes(ups, cs, tx, ty);
             if (tid < 2 * QY) colsum_lanes(ups, cs, QX + (tid & 1), tid >> 1);  // the two columns right of the last quad
         }
@@ -329,14 +331,18 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 4) k_collapse_tile(const
                 wt[q] = unit ? 1.f : fmul((float)(p[q] >> 24), SB_INV255);  // 255 * fl(1/255) == 1 exactly
             }
         } else {
-            const int sw = ((tile_x - o.x) & 3) + 2 * tx;  // the staged weight window starts at a multiple of 4 columns
+            const int sw = ((tile_x - o.x) & 3) + 2 * tx;  // the staged windows start at a multiple of 4 columns
             const float2 w0 = *reinterpret_cast<const float2 *>(&B.w[2 * ty][sw]);
             const float2 w1 = *reinterpret_cast<const float2 *>(&B.w[2 * ty + 1][sw]);
-            const uint4 a = *reinterpret_cast<const uint4 *>(&B.own[2 * ty][2 * tx]);
-            const uint4 b = *reinterpret_cast<const uint4 *>(&B.own[2 * ty + 1][2 * tx]);
+            const uint2 a = *reinterpret_cast<const uint2 *>(&B.own[2 * ty][sw]);
+            const uint2 b = *reinterpret_cast<const uint2 *>(&B.own[2 * ty + 1][sw]);
             wt[0] = w0.x; wt[1] = w0.y; wt[2] = w1.x; wt[3] = w1.y;
-            g_rb[0] = a.x; g_g[0] = a.y; g_rb[1] = a.z; g_g[1] = a.w;
-            g_rb[2] = b.x; g_g[2] = b.y; g_rb[3] = b.z; g_g[3] = b.w;
+            const unsigned p[4] = {a.x, a.y, b.x, b.y};
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                g_rb[q] = p[q] & 0x00ff00ffu;
+                g_g[q] = __byte_perm(p[q], 0u, 0x4441);
+            }
             nothing = wt[0] == 0.f && wt[1] == 0.f && wt[2] == 0.f && wt[3] == 0.f;
             unit = wt[0] == 1.f && wt[1] == 1.f && wt[2] == 1.f && wt[3] == 1.f;
         }

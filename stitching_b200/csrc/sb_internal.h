@@ -98,11 +98,13 @@ inline size_t warp_table_floats(int w, int h) { return (size_t)2 * ((w + 3) & ~3
 
 // one pyramid level of one fed image: planar int16 x3 + float32 weights
 // Two colour layouts.  An image fed as bytes (RGBM) keeps every Gaussian level inside 0..255 (the 5x5 weights sum
-// to 256), so its levels are stored as LANE PAIRS: q[y*pitch + x] = (r | b << 16, g), 8 bytes per pixel -- red and
-// blue travel as two 16-bit lanes of one word through every filter (no lane ever carries: 256*255+128 < 2^16).
+// to 256), so its levels are stored as ONE WORD per pixel: q[y*pitch + x] = r | g << 8 | b << 16, byte 3 zero --
+// the layout of level 0 without the mask byte.  The kernels split a word into two 16-bit lanes (r | b << 16 and g)
+// after loading it, and red and blue run as the two lanes of one word through every filter (no lane ever carries:
+// 256*255+128 < 2^16).
 // A generic int16 feed (arbitrary values) keeps planar int16 and is served by the simple kernels only.
 struct Level {
-    uint2 *q;          // [h][pitch] lane pairs, or null
+    uint32_t *q;       // [h][pitch] words, or null
     int16_t *g;        // [3][h][pitch] planar, or null
     float *w;          // [h][pitch]
     int w_px, h_px;    // level size
@@ -135,11 +137,11 @@ struct alignas(16) ColDesc {       // collapse of level l
     int ox, oy, w_l, h_l;          // padded rect of the image at level l, pano level coordinates
     const uint32_t *rgbm;          // level 0: packed fed image
     union {
-        const uint2 *q;            // kind 0, level l >= 1: colour lane pairs
+        const uint32_t *q;         // kind 0, level l >= 1: colour words
         const int16_t *g;          // kind 1: the slab's three int16 planes of partial sums
     };
     const float *w;                // weights (kind 1: weight sums)
-    const uint2 *uq;               // level l+1 colour lane pairs (null at the top level)
+    const uint32_t *uq;            // level l+1 colour words (null at the top level)
     int rgbm_pitch, iw, ih, left;  // level 0: image size and origin inside the padded rect
     int top, pitch, plane, upitch; // level l / l+1 pitches, in elements; plane: stride of a slab's planes
     int pad0, kind, pad1, pad2;    // kind 0: a fed image; 1: a slab of partial sums
@@ -147,9 +149,9 @@ struct alignas(16) ColDesc {       // collapse of level l
 struct alignas(16) PyrDesc {       // pyrDown of level l -> l+1
     int sw, sh, dpitch, pad3;      // source level size; destination pitch (elements)
     const uint32_t *rgbm;          // level 0 source
-    const uint2 *sq;               // level >= 1 source lane pairs
+    const uint32_t *sq;            // level >= 1 source colour words
     const float *swt;
-    uint2 *dq;
+    uint32_t *dq;
     float *dwt;
     int rgbm_pitch, iw;
     int ih, left, top, spitch;

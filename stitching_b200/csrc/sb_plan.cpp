@@ -187,8 +187,8 @@ int BlendPlan::allocate(cudaStream_t s)
             if (!active(i)) continue;  // another rank owns this image: geometry only
             for (int l = 1; l <= nb; ++l) {
                 const int w = imgs[i].pw >> l, h = imgs[i].ph >> l, pitch = level_pitch(w);
-                // byte-fed images: lane pairs (8 bytes per pixel); generic int16 feeds: three int16 planes
-                slots[i][l].g = carve(imgs[i].rgbm ? (size_t)h * pitch * sizeof(uint2) : (size_t)3 * h * pitch * sizeof(int16_t));
+                // byte-fed images: one word per pixel; generic int16 feeds: three int16 planes
+                slots[i][l].g = carve(imgs[i].rgbm ? (size_t)h * pitch * sizeof(uint32_t) : (size_t)3 * h * pitch * sizeof(int16_t));
                 slots[i][l].w = carve((size_t)h * pitch * sizeof(float));
             }
         }
@@ -224,7 +224,7 @@ int BlendPlan::allocate(cudaStream_t s)
                 L.h_px = imgs[i].ph >> l;
                 L.pitch = level_pitch(L.w_px);
                 L.plane = (long long)L.h_px * L.pitch;
-                L.q = active(i) && imgs[i].rgbm ? (uint2 *)(base + slots[i][l].g) : nullptr;
+                L.q = active(i) && imgs[i].rgbm ? (uint32_t *)(base + slots[i][l].g) : nullptr;
                 L.g = active(i) && !imgs[i].rgbm ? (int16_t *)(base + slots[i][l].g) : nullptr;
                 L.w = active(i) ? (float *)(base + slots[i][l].w) : nullptr;
             }
@@ -393,8 +393,8 @@ int BlendPlan::run(const PanoOut &out, cudaStream_t s, const std::function<int(c
     return SB_OK;
 }
 
-// Compulsory HBM traffic of this plan's kernels (every input byte read once, every output byte written
-// once, no accumulator round trips): see DESIGN.md "byte model".  Same order as run()'s launches.
+// Compulsory HBM traffic of this plan's kernels in the layouts the levels are stored in (every input byte read once,
+// every output byte written once, no accumulator round trips): see DESIGN.md "byte model".  Same order as run()'s launches.
 std::vector<std::pair<std::string, double>> BlendPlan::launch_bytes() const
 {
     std::vector<std::pair<std::string, double>> v;
@@ -405,12 +405,16 @@ std::vector<std::pair<std::string, double>> BlendPlan::launch_bytes() const
 #else
         const int T = tail_from <= nb ? tail_from : nb + 1;
 #endif
+        // bytes per pixel of a level >= 1 (colours + weight) and of its colours alone: one word + a float for byte-fed
+        // images, three int16 + a float for generic int16 feeds
+        auto lv_px = [](const FeedImage &im) { return im.rgbm ? 4.0 + 4.0 : 6.0 + 4.0; };
+        auto rgb_px = [](const FeedImage &im) { return im.rgbm ? 4.0 : 6.0; };
         double tail = 0;
         for (int l = 0; l < nb; ++l) {
             double b = 0;
             for (const FeedImage &im : imgs) {
                 const double src = (double)(im.pw >> l) * (im.ph >> l);
-                b += (l == 0 ? l0 : 10.0) * src + 10.0 * src / 4;  // read level l, write level l+1
+                b += (l == 0 ? l0 : lv_px(im)) * src + lv_px(im) * src / 4;  // read level l, write level l+1
             }
             if (l >= T)
                 tail += b;
@@ -421,8 +425,8 @@ std::vector<std::pair<std::string, double>> BlendPlan::launch_bytes() const
             double b = 0;
             for (const FeedImage &im : imgs) {
                 const double a = (double)(im.pw >> l) * (im.ph >> l);
-                b += (l == 0 ? l0 : 10.0) * a;   // G_l, W_l
-                if (l < nb) b += 6.0 * a / 4;    // G_{l+1} for the pyrUp
+                b += (l == 0 ? l0 : lv_px(im)) * a;   // G_l, W_l
+                if (l < nb) b += rgb_px(im) * a / 4;  // G_{l+1} for the pyrUp
             }
             const double P = (double)(wp >> l) * (hp >> l);
             if (l < nb) b += 6.0 * P / 4;        // C_{l+1}

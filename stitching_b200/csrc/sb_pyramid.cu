@@ -37,7 +37,7 @@ int launch_pyrdown(const FeedImage *imgs_dev, const FeedImage *imgs_host, const 
 {
     // max_w / max_h: largest DESTINATION level size among the images of the batch
     if (count <= 0 || max_w <= 0 || max_h <= 0) return SB_OK;
-    // the fast kernel works on byte-fed images (RGBM level 0, lane-pair levels); generic int16 feeds use the gather kernel
+    // the fast kernel works on byte-fed images (RGBM level 0, one colour word per pixel above); generic int16 feeds use the gather kernel
     bool packed = true;
     for (int i = first; i < first + count; ++i) packed = packed && imgs_host[i].rgbm != nullptr;
 #ifdef SB_EMU

@@ -38,14 +38,14 @@ __device__ __forceinline__ void load_level0(const FeedImage &im, int X, int Y, i
     wt = inside ? fmul((float)m, SB_INV255) : 0.f;
 }
 
-// the three colours of element o of a level >= 1, either layout (sb_internal.h: lane pairs or planar int16)
+// the three colours of element o of a level >= 1, either layout (sb_internal.h: one word per pixel or planar int16)
 __device__ __forceinline__ void load_colours(const Level &L, long long o, int c[3])
 {
     if (L.q) {
-        const uint2 v = L.q[o];
-        c[0] = (int)(v.x & 0xffffu);
-        c[1] = (int)v.y;
-        c[2] = (int)(v.x >> 16);
+        const unsigned v = L.q[o];
+        c[0] = (int)(v & 255u);
+        c[1] = (int)((v >> 8) & 255u);
+        c[2] = (int)(v >> 16);
     } else {
         c[0] = L.g[o];
         c[1] = L.g[L.plane + o];
@@ -55,7 +55,7 @@ __device__ __forceinline__ void load_colours(const Level &L, long long o, int c[
 __device__ __forceinline__ void store_colours(const Level &L, long long o, const int c[3])
 {
     if (L.q) {
-        L.q[o] = make_uint2((unsigned)c[0] | ((unsigned)c[2] << 16), (unsigned)c[1]);  // bytes: see sb_internal.h
+        L.q[o] = (unsigned)c[0] | ((unsigned)c[1] << 8) | ((unsigned)c[2] << 16);  // bytes: see sb_internal.h
     } else {
         L.g[o] = (int16_t)c[0];
         L.g[L.plane + o] = (int16_t)c[1];

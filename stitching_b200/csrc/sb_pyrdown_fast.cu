@@ -16,8 +16,9 @@
 //     filter passes (5x5 weights sum to 256, 256*255+128 < 2^16, so a lane never carries into its neighbour);
 //     each lane converts its own two mask bytes to float (2^23 mantissa trick, exact, keeps the XU pipe free) and
 //     the weights travel by shuffle as well;
-//   levels >= 1 (lane pairs r|b<<16, g per pixel + float32 weights): the own pair is one 16-byte load and the colours
-//     run through the same two-lane arithmetic; every level is written as lane pairs (one 8-byte store per pixel).
+//   levels >= 1 (one word r | g<<8 | b<<16 per pixel + float32 weights): the own pair is one 8-byte load of words
+//     (plus one of weights); a lane shuffles one word per tap and splits it into the r|b and g lanes after the
+//     shuffle, as at level 0; every level is written as one word per pixel (the two lanes packed back, one 4-byte store).
 // The float summation orders (position dependent, sb_pyramid.cuh) are per-lane constants.
 //
 // BIN (level 0, every mask byte of the batch is 0 or 255 -- the warped validity masks of a compositor without blend
@@ -49,7 +50,7 @@ __device__ __forceinline__ float byte3_to_float(unsigned p)
 
 struct Raw0 { unsigned p2, p3; };                 // own pair of packed pixels (mask byte cleared outside the image)
 struct H0 { unsigned rb, gm; float w; };
-struct Raw1 { uint2 p2, p3; float2 wp; };         // own pair of lane-pair pixels + weights
+struct Raw1 { unsigned p2, p3; float2 wp; };      // own pair of colour words + weights
 struct H1 { unsigned rb, g; float w; };
 
 // NEAR: every row index the walk produces is at most one reflection away from its range (the launcher checks the
@@ -73,9 +74,9 @@ __global__ void __launch_bounds__(32 * WK_WARPS, (L0 && BIN) ? 12 : 10) k_pyrdow
     const int4 db = __ldg(reinterpret_cast<const int4 *>(&D.ih));          // ih, left, top, spitch
     const int2 dc = __ldg(reinterpret_cast<const int2 *>(&D.rgbm_pitch));  // rgbm_pitch, iw
     const uint32_t *__restrict__ rgbm = D.rgbm;
-    const uint2 *__restrict__ sq = D.sq;
+    const uint32_t *__restrict__ sq = D.sq;
     const float *__restrict__ swt = D.swt;
-    uint2 *__restrict__ dq = D.dq;
+    uint32_t *__restrict__ dq = D.dq;
     float *__restrict__ dwt = D.dwt;
     const int ih = db.x, left = db.y, top = db.z, spitch = db.w, rgbm_pitch = dc.x, iw = dc.y;
 
@@ -125,10 +126,10 @@ __global__ void __launch_bounds__(32 * WK_WARPS, (L0 && BIN) ? 12 : 10) k_pyrdow
     auto fetch1 = [&](int src_row) -> Raw1 {
         const int ro = (NEAR ? reflect101_once(src_row, sh) : reflect101(src_row, sh)) * spitch;
         Raw1 r;
-        if (pair_adjacent) {  // (2x, 2x+1): one 16-byte / 8-byte load (true for every real column)
-            const uint4 v = __ldg(reinterpret_cast<const uint4 *>(sq + ro + c2));
-            r.p2 = make_uint2(v.x, v.y);
-            r.p3 = make_uint2(v.z, v.w);
+        if (pair_adjacent) {  // (2x, 2x+1): two 8-byte loads (true for every real column)
+            const uint2 v = __ldg(reinterpret_cast<const uint2 *>(sq + ro + c2));
+            r.p2 = v.x;
+            r.p3 = v.y;
             r.wp = __ldg(reinterpret_cast<const float2 *>(swt + ro + c2));
         } else {              // a reflected virtual column
             r.p2 = __ldg(sq + ro + c2);
@@ -139,15 +140,13 @@ __global__ void __launch_bounds__(32 * WK_WARPS, (L0 && BIN) ? 12 : 10) k_pyrdow
         return r;
     };
     auto hpass1 = [&](const Raw1 &r) -> H1 {
+        const unsigned p0 = __shfl_up_sync(FULL, r.p2, 1), p1 = __shfl_up_sync(FULL, r.p3, 1);
+        const unsigned p4 = __shfl_down_sync(FULL, r.p2, 1);
+        const unsigned M = 0x00ff00ffu;
         H1 h;
-        {
-            const unsigned p0 = __shfl_up_sync(FULL, r.p2.x, 1), p1 = __shfl_up_sync(FULL, r.p3.x, 1), p4 = __shfl_down_sync(FULL, r.p2.x, 1);
-            h.rb = p0 + p4 + 4u * (p1 + r.p3.x) + 6u * r.p2.x;
-        }
-        {
-            const unsigned p0 = __shfl_up_sync(FULL, r.p2.y, 1), p1 = __shfl_up_sync(FULL, r.p3.y, 1), p4 = __shfl_down_sync(FULL, r.p2.y, 1);
-            h.g = p0 + p4 + 4u * (p1 + r.p3.y) + 6u * r.p2.y;
-        }
+        h.rb = (p0 & M) + (p4 & M) + 4u * ((p1 & M) + (r.p3 & M)) + 6u * (r.p2 & M);
+        h.g = __byte_perm(p0, 0u, 0x4441) + __byte_perm(p4, 0u, 0x4441) +
+              4u * (__byte_perm(p1, 0u, 0x4441) + __byte_perm(r.p3, 0u, 0x4441)) + 6u * __byte_perm(r.p2, 0u, 0x4441);
         const float w0 = __shfl_up_sync(FULL, r.wp.x, 1), w1 = __shfl_up_sync(FULL, r.wp.y, 1);
         const float w4 = __shfl_down_sync(FULL, r.wp.x, 1);
         h.w = tap5_h(w0, w1, r.wp.x, r.wp.y, w4, BIN ? true : h_simd);
@@ -169,7 +168,7 @@ __global__ void __launch_bounds__(32 * WK_WARPS, (L0 && BIN) ? 12 : 10) k_pyrdow
                 const unsigned vrb = h0.rb + h4.rb + 4u * (h1.rb + h3.rb) + 6u * h2.rb + 0x00800080u;
                 const unsigned vgm = h0.gm + h4.gm + 4u * (h1.gm + h3.gm) + 6u * h2.gm + 0x00800080u;
                 const int o = y * dpitch + x;
-                dq[o] = make_uint2((vrb >> 8) & 0x00ff00ffu, (vgm >> 8) & 0xffu);
+                dq[o] = ((vrb >> 8) & 0x00ff00ffu) | (vgm & 0xff00u);  // green's lane is below 2^16: its bits 8..15 are g
                 if (BIN) {
                     const unsigned vm = (vgm >> 16) - 128u;                    // 255 * (filtered mask bits), <= 65280
                     dwt[o] = fmul((float)((vm * 257u + 65535u) >> 16), 0.00390625f);
@@ -197,7 +196,7 @@ __global__ void __launch_bounds__(32 * WK_WARPS, (L0 && BIN) ? 12 : 10) k_pyrdow
                 const unsigned vrb = h0.rb + h4.rb + 4u * (h1.rb + h3.rb) + 6u * h2.rb + 0x00800080u;
                 const unsigned vg = h0.g + h4.g + 4u * (h1.g + h3.g) + 6u * h2.g + 128u;
                 const int o = y * dpitch + x;
-                dq[o] = make_uint2((vrb >> 8) & 0x00ff00ffu, vg >> 8);
+                dq[o] = ((vrb >> 8) & 0x00ff00ffu) | (vg & 0xff00u);  // vg < 2^16: its bits 8..15 are g
                 dwt[o] = tap5_v(h0.w, h1.w, h2.w, h3.w, h4.w, BIN ? true : v_simd);
             }
             h0 = h2;
