@@ -183,7 +183,21 @@ typedef struct {
 
 SB_API sb_compositor *sb_compositor_create(const sb_rig *rig);
 SB_API void sb_compositor_destroy(sb_compositor *c);
-/* geometry of the plan: per image warped rect {x,y,w,h} (== sb_warp_roi) and the pano roi {x,y,w,h} */
+
+/* The crop of Stitcher's default Cropper (cropper.py), in FINAL pixels: image i feeds the slice `rect` of its warped
+ * image at `corner`, and Blender.prepare sees `size`.  The pano roi and num_bands follow the prepared sizes. */
+typedef struct {
+    const int *rect;    /* [n][4] x, y, w, h in warped image i's own pixels: the slice cropper.py:150-151 takes
+                           (clipped like a numpy slice by the library) */
+    const int *corner;  /* [n][2] Blender.feed corner of image i (Cropper.crop_rois) */
+    const int *size;    /* [n][2] size of image i as Blender.prepare receives it (Cropper.crop_rois) */
+} sb_crop;
+/* sb_compositor_create (world == 1) or sb_compositor_create_sharded with a crop; crop == NULL crops nothing.  A negative
+ * offset or size, an empty slice or a slice larger than its prepared size fails (SB_ERR_INVALID, named in sb_last_error):
+ * the reference's blenders cannot feed an empty image either. */
+SB_API sb_compositor *sb_compositor_create_cropped(const sb_rig *rig, const sb_crop *crop, int rank, int world);
+/* geometry of the plan: per image warped rect {x,y,w,h} (== sb_warp_roi; with a crop: feed corner and fed size) and the
+ * pano roi {x,y,w,h} */
 SB_API int sb_compositor_geometry(const sb_compositor *c, int *rects /*[n][4]*/, int pano_roi[4], int *num_bands);
 /* compulsory HBM traffic of one run (DESIGN.md byte model) for the roofline: total, and per kernel launch in
  * launch order (same order as sb_compositor_stage_times).  Returns the number of launches (or < 0). */

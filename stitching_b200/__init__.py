@@ -7,7 +7,7 @@ unchanged.
 """
 from . import exposure_error_compensator, images, seam_finder  # noqa: F401
 from .blender import Blender  # noqa: F401
-from .compositor import Compositor  # noqa: F401
+from .compositor import Compositor, Crop  # noqa: F401
 from .stitching_error import StitchingError, StitchingWarning  # noqa: F401
 from .timelapser import Timelapser  # noqa: F401
 from .warper import Warper  # noqa: F401

@@ -42,6 +42,10 @@ class Rig(C.Structure):
     ]
 
 
+class CropDesc(C.Structure):
+    _fields_ = [("rect", c_int_p), ("corner", c_int_p), ("size", c_int_p)]
+
+
 # every symbol include/stitch_b200.h declares: (name, restype, argtypes)
 SIGNATURES = [
     ("sb_last_error", C.c_char_p, []),
@@ -90,6 +94,7 @@ SIGNATURES = [
     ("sb_compositor_time_multi", C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, c_float_p]),
     ("sb_compositor_stage_times", C.c_int, [C.c_void_p, C.POINTER(C.c_char_p), c_float_p, C.c_int]),
     ("sb_compositor_create_sharded", C.c_void_p, [C.POINTER(Rig), C.c_int, C.c_int]),
+    ("sb_compositor_create_cropped", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), C.c_int, C.c_int]),
     ("sb_compositor_shard_info", C.c_int, [C.c_void_p, c_int_p, c_int_p, c_int_p]),
     ("sb_compositor_shard_phase", C.c_int, [C.c_void_p, C.c_int]),
     ("sb_compositor_shard_slab", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]),

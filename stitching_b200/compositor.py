@@ -1,9 +1,10 @@
 """Fused warp + blend on one GPU with every intermediate resident in HBM (sb_compositor_* in the C ABI).
 
-Equivalent to running, for a fixed rig, stitcher.py:178-189 (Warper.warp_images / create_and_warp_masks /
-warp_rois at final resolution) and stitcher.py:241-259 (Blender.prepare / feed / blend) -- with the warped
-validity mask as blend mask (seam finder "no") -- but with one host->device copy of the sources and one
-device->host copy of the panorama.
+Equivalent to running, for a fixed rig, the FINAL-resolution half of Stitcher.stitch: stitcher.py:178-189
+(Warper.warp_images / create_and_warp_masks / warp_rois), the crop of stitcher.py:198-208 when a `Crop` is given,
+ExposureErrorCompensator.apply and SeamFinder.resize when gains and seam masks are set, and stitcher.py:241-259
+(Blender.prepare / feed / blend) -- with one host->device copy of the sources and one device->host copy of the
+panorama.  Without seam masks or masks the warped validity mask is the blend mask (seam finder "no").
 """
 import ctypes as C
 from statistics import median
@@ -24,10 +25,50 @@ def time_multi(compositors, iters):
     return ms.value
 
 
+def _scaled(rect, aspect):
+    """A LOW-resolution (x, y, w, h) in FINAL pixels, each component rounded half to even (Python's round)."""
+    return tuple(int(round(v * aspect)) for v in rect)
+
+
+class Crop:
+    """The crop of every image in FINAL pixels, as Stitcher.crop_final_resolution applies it.
+
+    rects[i]: (x, y, w, h), the slice of warped image i that is fed (clipped at the warped image's bottom and right);
+    corners[i]: where it is fed (Blender.feed); sizes[i]: its size as Blender.prepare sees it, which sets the pano roi
+    and num_bands.  The fed size is the clipped slice, so it may be smaller than sizes[i]."""
+
+    def __init__(self, rects, corners, sizes):
+        self.rects = [tuple(int(v) for v in r) for r in rects]
+        self.corners = [tuple(int(v) for v in c) for c in corners]
+        self.sizes = [tuple(int(v) for v in s) for s in sizes]
+        if not (len(self.rects) == len(self.corners) == len(self.sizes)):
+            raise StitchingError("Crop needs one rect, corner and size per image")
+        if any(len(r) != 4 for r in self.rects) or any(len(c) != 2 for c in self.corners) or any(len(s) != 2 for s in self.sizes):
+            raise StitchingError("Crop: rects are (x, y, w, h), corners (x, y), sizes (w, h)")
+
+    @classmethod
+    def from_cropper(cls, cropper, aspect=1):
+        """The crop a prepared Cropper (cropper.py) applies at `aspect` = LOW -> FINAL ratio; None if it does not crop.
+
+        Image i is sliced by its intersection rectangle and fed at its overlapping rectangle, both scaled separately
+        (so their roundings differ); the scaled overlap corners are shifted so that the smallest x and y are 0."""
+        if not cropper.do_crop:
+            return None
+        rects = [_scaled(r, aspect) for r in cropper.intersection_rectangles]
+        overlaps = [_scaled(r, aspect) for r in cropper.overlapping_rectangles]
+        x0 = min(o[0] for o in overlaps)
+        y0 = min(o[1] for o in overlaps)
+        return cls(rects, [(o[0] - x0, o[1] - y0) for o in overlaps], [(o[2], o[3]) for o in overlaps])
+
+
 class Compositor:
     def __init__(self, cameras, sizes, warper_type="spherical", blender_type="multiband", blend_strength=5, scale=None,
-                 aspect=1, rank=0, world=1):
+                 aspect=1, rank=0, world=1, crop=None):
         """cameras: objects with .focal, .K(), .R (cv.detail.CameraParams or rigs.Camera); sizes: [(w, h)].
+
+        crop: a `Crop` (e.g. Crop.from_cropper(stitcher.cropper, aspect)); every image is then warped only over its
+        slice and fed at the crop's corner, and `self.rects` holds the fed rects (corner, fed size): the shapes that
+        set_mask and download_warped use, and that set_seam_mask and set_gain resize to.
 
         world > 1: one panorama over `world` GPUs, one process per GPU.  Every rank passes ALL cameras; rank r owns
         images [r*n/world, (r+1)*n/world) -- `self.first`, `self.count` -- uploads only those and gets the column
@@ -35,6 +76,8 @@ class Compositor:
         n = len(cameras)
         if n == 0 or len(sizes) != n:
             raise StitchingError("Compositor needs one size per camera")
+        if crop is not None and len(crop.rects) != n:
+            raise StitchingError(f"Crop has {len(crop.rects)} rects for {n} images")
         if warper_type not in _lib.WARP_TYPES:
             raise StitchingError(f"warper type '{warper_type}' is not on the GPU path")
         if blender_type not in _lib.BLEND_KINDS:
@@ -53,7 +96,11 @@ class Compositor:
                        self._R.ctypes.data_as(_lib.c_float_p), 0)
         L = self._L = _lib.lib()  # close() releases through the library that created the compositor
         self.rank, self.world = int(rank), int(world)
-        if self.world > 1:
+        if crop is not None:
+            arrs = [(C.c_int * (k * n))(*[v for t in ts for v in t]) for k, ts in ((4, crop.rects), (2, crop.corners), (2, crop.sizes))]
+            desc = _lib.CropDesc(*[C.cast(a, _lib.c_int_p) for a in arrs])
+            self._c = L.sb_compositor_create_cropped(C.byref(rig), C.byref(desc), self.rank, self.world)
+        elif self.world > 1:
             self._c = L.sb_compositor_create_sharded(C.byref(rig), self.rank, self.world)
         else:
             self._c = L.sb_compositor_create(C.byref(rig))

@@ -140,7 +140,36 @@ static void compositor_free(sb_compositor *c)
     delete c;
 }
 
-static int compositor_build(sb_compositor *c, const sb_rig *rig, int rank, int world)
+// What image i feeds with a crop (Stitcher.crop_final_resolution): the slice rect = (x, y, w, h) of its warped image,
+// clipped at the bottom and right like a numpy slice, is warped -- `proj` in pano-absolute coordinates -- and fed at
+// (corner, fed size); the prepared size only enters the pano roi.  The rounding of the two scaled rectangles differs, so
+// neither the slice nor the corner can be derived from the other.
+static int crop_image(const sb_crop *crop, int i, const Rect &warped, Rect *proj, Rect *placed, int prepared[2])
+{
+    const int *r = crop->rect + 4 * i;
+    const int *sz = crop->size + 2 * i;
+    if (r[0] < 0 || r[1] < 0 || r[2] < 0 || r[3] < 0 || sz[0] < 0 || sz[1] < 0) {
+        set_error("compositor: crop of image %d has a negative offset or size (%d,%d %dx%d, size %dx%d)", i, r[0], r[1], r[2], r[3], sz[0], sz[1]);
+        return SB_ERR_INVALID;
+    }
+    const int w = std::max(0, std::min(r[2], warped.w - r[0])), h = std::max(0, std::min(r[3], warped.h - r[1]));
+    if (w == 0 || h == 0) {
+        // the reference's blenders cannot take an empty image either: feed asserts (no, feather) or never returns (multiband)
+        set_error("compositor: crop of image %d is empty (%d,%d %dx%d of a %dx%d warped image)", i, r[0], r[1], r[2], r[3], warped.w, warped.h);
+        return SB_ERR_INVALID;
+    }
+    if (w > sz[0] || h > sz[1]) {
+        set_error("compositor: crop of image %d feeds %dx%d, more than its prepared size %dx%d", i, w, h, sz[0], sz[1]);
+        return SB_ERR_INVALID;
+    }
+    *proj = Rect{warped.x + r[0], warped.y + r[1], w, h};
+    *placed = Rect{crop->corner[2 * i], crop->corner[2 * i + 1], w, h};
+    prepared[0] = sz[0];
+    prepared[1] = sz[1];
+    return SB_OK;
+}
+
+static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *crop, int rank, int world)
 {
     const int n = rig->n_images;
     c->n = n;
@@ -182,6 +211,16 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, int rank, int w
         corners[2 * i + 1] = rect[1];
         sizes[2 * i] = rect[2];
         sizes[2 * i + 1] = rect[3];
+        if (crop) {  // from here on `rect` is the part of the warped rect that is warped and fed, c->rects[i] where it is fed
+            Rect proj;
+            SB_TRY(crop_image(crop, i, c->rects[i], &proj, &c->rects[i], &sizes[2 * i]));
+            rect[0] = proj.x;
+            rect[1] = proj.y;
+            rect[2] = proj.w;
+            rect[3] = proj.h;
+            corners[2 * i] = c->rects[i].x;
+            corners[2 * i + 1] = c->rects[i].y;
+        }
         c->max_w = std::max(c->max_w, rect[2]);
         c->max_h = std::max(c->max_h, rect[3]);
         if (!mine(i)) continue;  // another rank warps this image: only its geometry is needed here
@@ -519,10 +558,10 @@ static bool valid_rig(const sb_rig *rig)
            rig->blend_kind <= SB_BLEND_MULTIBAND;
 }
 
-static sb_compositor *compositor_create(const sb_rig *rig, int rank, int world)
+static sb_compositor *compositor_create(const sb_rig *rig, const sb_crop *crop, int rank, int world)
 {
     sb_compositor *c = new sb_compositor;
-    if (compositor_build(c, rig, rank, world) != SB_OK) {
+    if (compositor_build(c, rig, crop, rank, world) != SB_OK) {
         compositor_free(c);
         return nullptr;
     }
@@ -537,7 +576,7 @@ sb_compositor *sb_compositor_create(const sb_rig *rig)
         set_error("sb_compositor_create: invalid rig");
         return nullptr;
     }
-    return compositor_create(rig, 0, 1);
+    return compositor_create(rig, nullptr, 0, 1);
 }
 
 // One panorama over `world` GPUs (one process each): this rank warps and pyramids images
@@ -548,7 +587,17 @@ sb_compositor *sb_compositor_create_sharded(const sb_rig *rig, int rank, int wor
         set_error("sb_compositor_create_sharded: invalid argument");
         return nullptr;
     }
-    return compositor_create(rig, rank, world);
+    return compositor_create(rig, nullptr, rank, world);
+}
+
+// Either of the two above, with every image cropped as Stitcher.crop_final_resolution does (crop_image)
+sb_compositor *sb_compositor_create_cropped(const sb_rig *rig, const sb_crop *crop, int rank, int world)
+{
+    if (!valid_rig(rig) || world < 1 || rank < 0 || rank >= world || (crop && (!crop->rect || !crop->corner || !crop->size))) {
+        set_error("sb_compositor_create_cropped: invalid argument");
+        return nullptr;
+    }
+    return compositor_create(rig, crop, rank, world);
 }
 
 int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_local, int strip[2])
