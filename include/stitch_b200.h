@@ -98,7 +98,8 @@ SB_API int sb_seam_resize(const uint8_t *seam, size_t seam_pitch, int sw, int sh
  * warper.py:58-68 create_and_warp_mask -> PyRotationWarper.warp(INTER_NEAREST, BORDER_CONSTANT) on a 255 mask
  * Both outputs come from ONE kernel pass.  dst_img / dst_mask may each be NULL; their extents must be
  * out_rect[3] rows x out_rect[2] columns as given by sb_warp_roi for the same arguments.
- * src may be NULL when dst_img is NULL (mask only needs the source size). */
+ * src may be NULL when dst_img is NULL (mask only needs the source size).  A source or result with a side of 32767 px or
+ * more fails with SB_ERR_INVALID, as cv::remap asserts; with both outputs NULL only out_rect is computed (warpRoi). */
 SB_API int sb_warp(int warp_type, float scale, const float K[9], const float R[9], const uint8_t *src, int src_w,
                    int src_h, size_t src_pitch, uint8_t *dst_img, size_t dst_pitch, uint8_t *dst_mask,
                    size_t mask_pitch, int out_rect[4]);
@@ -173,7 +174,8 @@ typedef struct {
     int warp_type;        /* sb_warp_type */
     float scale;          /* Warper.scale * aspect (warper.py:44) */
     int blend_kind;       /* sb_blend_kind */
-    float blend_strength; /* blender.py:14 DEFAULT_BLEND_STRENGTH = 5; num_bands / sharpness derived as blender.py:25-36 */
+    double blend_strength; /* blender.py:14 DEFAULT_BLEND_STRENGTH = 5; num_bands / sharpness derived as blender.py:25-36,
+                              in double like the reference's Python float (a float32 strength moves both) */
     const int *src_w;     /* [n] */
     const int *src_h;     /* [n] */
     const float *K;       /* [n][9] */

@@ -13,6 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libstitch_b200.so")
 
 SB_OK = 0
+SB_ERR_INVALID = -1
 WARP_TYPES = {  # warper.py:10-27 -> sb_warp_type
     "spherical": 0, "cylindrical": 1, "plane": 2, "affine": 3, "fisheye": 4, "stereographic": 5,
     "compressedPlaneA2B1": 6, "compressedPlaneA1.5B1": 7, "compressedPlanePortraitA2B1": 8, "compressedPlanePortraitA1.5B1": 9,
@@ -33,7 +34,7 @@ class Rig(C.Structure):
         ("warp_type", C.c_int),
         ("scale", C.c_float),
         ("blend_kind", C.c_int),
-        ("blend_strength", C.c_float),
+        ("blend_strength", C.c_double),
         ("src_w", c_int_p),
         ("src_h", c_int_p),
         ("K", c_float_p),

@@ -92,7 +92,7 @@ class Compositor:
         self._w = (C.c_int * n)(*[s[0] for s in self.sizes])
         self._h = (C.c_int * n)(*[s[1] for s in self.sizes])
         rig = _lib.Rig(n, _lib.WARP_TYPES[warper_type], np.float32(self.scale), _lib.BLEND_KINDS[blender_type],
-                       np.float32(blend_strength), self._w, self._h, self._K.ctypes.data_as(_lib.c_float_p),
+                       float(blend_strength), self._w, self._h, self._K.ctypes.data_as(_lib.c_float_p),
                        self._R.ctypes.data_as(_lib.c_float_p), 0)
         L = self._L = _lib.lib()  # close() releases through the library that created the compositor
         self.rank, self.world = int(rank), int(world)

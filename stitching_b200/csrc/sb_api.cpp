@@ -166,6 +166,13 @@ static int warp_impl(int warp_type, float scale, const float K[9], const float R
         set_error("sb_warp: destination pitch too small for roi width %d", w);
         return SB_ERR_INVALID;
     }
+    // cv::remap asserts that both images are narrower and lower than SHRT_MAX (the warp of the image and the warp of the
+    // mask alike); warpRoi does not, so the roi-only call above still answers
+    if (src_w >= SB_MAX_WARP_SIDE || src_h >= SB_MAX_WARP_SIDE || w >= SB_MAX_WARP_SIDE || h >= SB_MAX_WARP_SIDE) {
+        set_error("sb_warp: source %dx%d or result %dx%d has a side of %d px or more, which cv::remap refuses", src_w, src_h, w, h,
+                  SB_MAX_WARP_SIDE);
+        return SB_ERR_INVALID;
+    }
     SB_TRY(ensure_device());
     cudaStream_t s = default_stream();
     Scratch tmp(s);

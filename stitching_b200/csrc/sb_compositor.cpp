@@ -206,6 +206,12 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *
             set_error("compositor: degenerate warped roi %dx%d for image %d", rect[2], rect[3], i);
             return SB_ERR_INVALID;
         }
+        // the reference warps every image whole (before any crop) with cv::remap, which refuses such sides
+        if (c->src_w[i] >= SB_MAX_WARP_SIDE || c->src_h[i] >= SB_MAX_WARP_SIDE || rect[2] >= SB_MAX_WARP_SIDE || rect[3] >= SB_MAX_WARP_SIDE) {
+            set_error("compositor: image %d (source %dx%d, warped %dx%d) has a side of %d px or more, which cv::remap refuses", i,
+                      c->src_w[i], c->src_h[i], rect[2], rect[3], SB_MAX_WARP_SIDE);
+            return SB_ERR_INVALID;
+        }
         c->rects[i] = Rect{rect[0], rect[1], rect[2], rect[3]};
         corners[2 * i] = rect[0];
         corners[2 * i + 1] = rect[1];

@@ -11,6 +11,9 @@
 #define SB_MAX_BANDS 16
 #define SB_MAX_IMAGES 256
 #define SB_SRC_PAD 16  // spare bytes after a source image: the warp kernel reads aligned 8-byte words
+// cv::remap (under PyRotationWarper.warp) asserts every side of its source and result below SHRT_MAX: the warp entries and
+// the compositor refuse sources and warped images with a side of this many pixels or more
+#define SB_MAX_WARP_SIDE 32767
 
 namespace sb {
 

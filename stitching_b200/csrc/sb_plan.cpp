@@ -29,10 +29,10 @@ Rect result_roi(const int *corners_xy, const int *sizes_wh, int n)
     return Rect{x0, y0, x1 - x0, y1 - y0};
 }
 
-void derive_blend_params(int requested_kind, float blend_strength, const Rect &roi, int *kind, int *num_bands, float *sharpness)
+void derive_blend_params(int requested_kind, double blend_strength, const Rect &roi, int *kind, int *num_bands, float *sharpness)
 {
     // blender.py:25  blend_width = sqrt(w*h) * strength / 100 (double)
-    const double blend_width = std::sqrt((double)roi.w * (double)roi.h) * (double)blend_strength / 100.0;
+    const double blend_width = std::sqrt((double)roi.w * (double)roi.h) * blend_strength / 100.0;
     *num_bands = 0;
     *sharpness = 0.f;
     if (requested_kind == SB_BLEND_NO || blend_width < 1.0) {

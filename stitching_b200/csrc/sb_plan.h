@@ -25,7 +25,7 @@ struct FeedDesc {
 };
 
 // derive blender.py:25-36's parameters: returns blend kind actually used and num_bands / sharpness
-void derive_blend_params(int requested_kind, float blend_strength, const Rect &roi, int *kind, int *num_bands, float *sharpness);
+void derive_blend_params(int requested_kind, double blend_strength, const Rect &roi, int *kind, int *num_bands, float *sharpness);
 Rect result_roi(const int *corners_xy, const int *sizes_wh, int n);  // cv.detail.resultRoi (blender.py:24)
 
 class BlendPlan {

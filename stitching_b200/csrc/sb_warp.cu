@@ -170,7 +170,9 @@ __device__ __forceinline__ void fetch_pair(const uint8_t *__restrict__ src, unsi
     }
 }
 
-// Generic fast variant (sb_warp with separate image / mask outputs, sources wider than int16): one pixel per thread.
+// Generic fast variant (sb_warp with separate image / mask outputs, the host-built maps, 1-px sources): one pixel per
+// thread.  Every side is below 32767 (SB_MAX_WARP_SIDE), so the int16 saturation only ever clamps coordinates that lie
+// outside the image.
 __global__ void __launch_bounds__(WARP_BX *WARP_BY) k_warp_wide(const __grid_constant__ WarpBatch B)
 {
     const WarpJob &j = B.j[blockIdx.z];

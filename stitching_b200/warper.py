@@ -119,15 +119,15 @@ class Warper:
         # Masks stay plain writable ndarrays: the reference hands them to cv2 calls that write into them
         # (seam_finder.py:35, the seam finders' find() modifies `masks` in place).
         keep_i = C.c_void_p()
-        _lib.check(
-            L.sb_warp_keep(
-                wtype, scale, _fp(K), _fp(R), src_p, int(size[0]), int(size[1]), pitch,
-                out.ctypes.data_as(C.c_void_p) if want_image else None, w * 3,
-                msk.ctypes.data_as(C.c_void_p) if want_mask else None, w, rect,
-                C.byref(keep_i) if want_image else None, None,
-            ),
-            "sb_warp_keep",
+        rc = L.sb_warp_keep(
+            wtype, scale, _fp(K), _fp(R), src_p, int(size[0]), int(size[1]), pitch,
+            out.ctypes.data_as(C.c_void_p) if want_image else None, w * 3,
+            msk.ctypes.data_as(C.c_void_p) if want_mask else None, w, rect,
+            C.byref(keep_i) if want_image else None, None,
         )
+        if rc == _lib.SB_ERR_INVALID:  # e.g. a side of 32767 px or more, where cv::remap asserts
+            raise _lib_argument_error("sb_warp_keep: " + L.sb_last_error().decode(errors="replace"))
+        _lib.check(rc, "sb_warp_keep")
         if want_image:
             out = device_array.wrap(out, keep_i.value)
         return out, msk

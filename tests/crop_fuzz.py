@@ -115,15 +115,16 @@ def named(name, budget):
 
 
 # -- the two sides ----------------------------------------------------------------------------------------------------
-def oracle_run(O, cc, imgs, ex):
+def oracle_run(O, cc, imgs, ex, s16=False):
     """Stitcher order: warp, slice image and mask (a numpy slice), compensator apply on the cropped image, blend mask =
     the caller's mask or SeamFinder.resize(seam, cropped mask) or the cropped mask; Blender.prepare(cropped corners,
-    sizes), feed at the cropped corners, blend."""
+    sizes), feed at the cropped corners, blend.  `raw` and "pano16" as in rig_fuzz.oracle_run."""
     case = cc.case
     scale = case.scale()
-    warped, masks = [], []
+    warped, masks, raw = [], [], []
     for img, cam, (x, y, w, h), (mask, seam, gain) in zip(imgs, case.cams, cc.crop.rects, ex):
         _, wi, wm = O.warp(case.wtype, scale, rig_fuzz.Warper.get_K(cam, 1), cam.R, img)
+        raw.append((wi, wm))
         wi = np.ascontiguousarray(wi[y:y + h, x:x + w])
         wm = np.ascontiguousarray(wm[y:y + h, x:x + w])
         if gain is not None:
@@ -138,10 +139,10 @@ def oracle_run(O, cc, imgs, ex):
     b.prepare(cc.crop.corners, cc.crop.sizes)
     for wi, wm, c in zip(warped, masks, cc.crop.corners):
         b.feed(wi, wm, c)
-    pano, pmask = b.blend()
+    pano16, pmask = b.blend_s16()
     rects = [tuple(c) + (wi.shape[1], wi.shape[0]) for c, wi in zip(cc.crop.corners, warped)]
     return dict(warped=warped, masks=masks, rects=rects, roi=b.roi, num_bands=b.num_bands if b._kind == "multiband" else -1,
-                pano=pano, pmask=pmask)
+                pano=O.convert_scale_abs(pano16), pmask=pmask, raw=raw, pano16=pano16 if s16 else None)
 
 
 def compositor(cc, crop=True, **kw):
@@ -195,7 +196,7 @@ def sharded_cases(seed, count, budget):
             cc = CropCase(c, Crop.from_cropper(cr, aspect), aspect)
             fed = cc.fed()
             _, _, w, h = _roi(cc.crop.corners, cc.crop.sizes)
-            blends = _bands(c, w, h) >= 1 if c.blender == "multiband" else math.sqrt(w * h) * float(np.float32(c.strength)) >= 100.0
+            blends = _bands(c, w, h) >= 1 if c.blender == "multiband" else math.sqrt(w * h) * c.strength >= 100.0
             if blends and all(f[2] > 0 and f[3] > 0 for f in fed) and \
                     _roi(cc.crop.corners, cc.crop.sizes) == _roi(cc.crop.corners, [f[2:] for f in fed]):
                 out.append(cc)
@@ -269,7 +270,7 @@ def _roi(corners, sizes):
 
 
 def _bands(case, w, h):
-    bw = math.sqrt(w * h) * float(np.float32(case.strength)) / 100.0
+    bw = math.sqrt(w * h) * case.strength / 100.0
     if case.blender != "multiband" or bw < 1.0:
         return -1
     return min(int(math.log(bw) / math.log(2.0) - 1.0), int(math.ceil(math.log(max(w, h)) / math.log(2.0))))

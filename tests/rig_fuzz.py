@@ -156,7 +156,8 @@ def _sizes(rng, n, side, small=False):
 
 
 def _quant(x):
-    """A float32-exact value, so that the compositor (float32 strength) and the oracle (double) see the same number."""
+    """`x` on a grid of 1/256 (float32-exact).  The compositor takes the strength in double like the oracle, so any
+    value would do; the grid stays so that the seeded draws do not move (tests/dropin_fuzz.py draws inexact ones)."""
     return float(np.float32(round(x * 256) / 256))
 
 
@@ -390,14 +391,16 @@ def redraw_share(cs):
 
 
 # -- the oracle side ----------------------------------------------------------------------------------------------------
-def oracle_run(O, case, imgs, ex):
+def oracle_run(O, case, imgs, ex, s16=False):
     """The reference order of operations per image (stitcher.py:178-189, 219-225, 241-259): warp, compensator apply on
     the warped image, blend mask = the caller's mask, or SeamFinder.resize(seam, warped mask), or the warped mask; then
-    Blender prepare / feed / blend."""
+    Blender prepare / feed / blend.  `raw` holds the warped images and masks before compensation; s16: also the blend's
+    int16 result ("pano16")."""
     scale = case.scale()
-    warped, masks, corners, sizes = [], [], [], []
+    warped, masks, corners, sizes, raw = [], [], [], [], []
     for img, cam, (mask, seam, gain) in zip(imgs, case.cams, ex):
         rect, wi, wm = O.warp(case.wtype, scale, Warper.get_K(cam, 1), cam.R, img)
+        raw.append((wi, wm))
         if gain is not None:
             wi = O.gain_apply(wi, gain)
         if mask is not None:
@@ -412,9 +415,10 @@ def oracle_run(O, case, imgs, ex):
     b.prepare(corners, sizes)
     for wi, wm, c in zip(warped, masks, corners):
         b.feed(wi, wm, c)
-    pano, pmask = b.blend()
+    pano16, pmask = b.blend_s16()
     return dict(warped=warped, masks=masks, rects=[tuple(c) + tuple(s) for c, s in zip(corners, sizes)], roi=b.roi,
-                num_bands=b.num_bands if b._kind == "multiband" else -1, pano=pano, pmask=pmask)
+                num_bands=b.num_bands if b._kind == "multiband" else -1, pano=O.convert_scale_abs(pano16), pmask=pmask,
+                raw=raw, pano16=pano16 if s16 else None)
 
 
 def compositor_run(Compositor, case, imgs, ex):
@@ -454,7 +458,7 @@ def check(case, got, ref, seed):
 def plan(case):
     """Blend kind, band count and the padded rects of a case, restated from sb_plan.cpp."""
     x, y, w, h = case.roi()
-    bw = math.sqrt(w * h) * float(np.float32(case.strength)) / 100.0  # derive_blend_params (sb_plan.cpp:32-47)
+    bw = math.sqrt(w * h) * case.strength / 100.0  # derive_blend_params (sb_plan.cpp:32-47)
     if case.blender == "no" or bw < 1.0:
         return "no", 0, []
     if case.blender == "feather":
