@@ -86,6 +86,9 @@ class Compositor:
         self.sizes = [(int(w), int(h)) for w, h in sizes]
         if scale is None:
             scale = median([cam.focal for cam in cameras])  # Warper.set_scale
+        # Stitcher's ratios are numpy float64, so Warper.get_K scales the float32 K in double and rounds once; a Python
+        # float would make numpy multiply in float32, one rounding off at some ratios.  Take the ratio as the Stitcher does.
+        aspect = np.float64(aspect)
         self.scale = scale * aspect
         self._K = np.ascontiguousarray(np.stack([Warper.get_K(c, aspect) for c in cameras]).astype(np.float32))
         self._R = np.ascontiguousarray(np.stack([np.asarray(c.R, np.float32) for c in cameras]))

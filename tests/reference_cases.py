@@ -198,6 +198,79 @@ def synthetic_scans(cv):
     return scans
 
 
+def _mix(a, b, salt):
+    """A 64-bit hash of integer cell coordinates (uint64 arithmetic wraps the same way on every machine)."""
+    with np.errstate(over="ignore"):
+        h = a.astype(np.uint64) * np.uint64(0x9E3779B97F4A7C15) + b.astype(np.uint64) * np.uint64(0xC2B2AE3D27D4EB4F) + np.uint64(salt)
+        h ^= h >> np.uint64(29)
+        h *= np.uint64(0xBF58476D1CE4E5B9)
+        h ^= h >> np.uint64(32)
+    return h
+
+
+def _byte(h, shift, lo, hi):
+    return (lo + ((h >> np.uint64(shift)) & np.uint64(255)).astype(np.int32) * (hi - lo) // 256).astype(np.int32)
+
+
+def _discs(u, v, cell, rmin, rmax, salt, out):
+    """One disc per `cell` x `cell` square of the scene, centre, radius and colour from the square's hash."""
+    cx, cy = np.floor(u / cell), np.floor(v / cell)
+    h = _mix(cx.astype(np.int64), cy.astype(np.int64), salt)
+    r = rmin + (rmax - rmin) * ((h & np.uint64(255)).astype(np.float64) / 255.0)
+    du = u - (cx + 0.5) * cell - (((h >> np.uint64(8)) & np.uint64(255)).astype(np.float64) - 127.5) * (cell / 2 - rmax) / 127.5
+    dv = v - (cy + 0.5) * cell - (((h >> np.uint64(16)) & np.uint64(255)).astype(np.float64) - 127.5) * (cell / 2 - rmax) / 127.5
+    inside = du * du + dv * dv < r * r
+    for ch in range(3):
+        out[..., ch] = np.where(inside, _byte(h, 24 + 8 * ch, 0, 256), out[..., ch])
+
+
+# Camera-resolution views: (tan of half the yaw step, exposure in percent) per view, left to right.  The yaws are
+# 2 atan(t); sin and cos are the rationals 2t / (1 + t^2) and (1 - t^2) / (1 + t^2), so no library trigonometry enters.
+CAMERA_VIEW_YAWS = {3: (-0.18, 0.0, 0.18), 4: (-0.16, -0.053, 0.053, 0.16)}
+CAMERA_VIEW_GAINS = {3: (82, 100, 112), 4: (82, 100, 112, 91)}
+
+
+def camera_views(w, h, n, seed):
+    """`n` views of w x h (camera resolution) of one textured plane, turned by yaw steps of 12 degrees (4 views) or 20
+    degrees (3 views), focal 0.9 w, at different exposures: the input of the recorded camera-resolution Stitcher runs.
+    Every pair of views overlaps, so that no pair is left to a chance match above the 0.3 confidence threshold.
+
+    Every pixel is rendered at this resolution from the plane point its ray meets -- blocks and two sizes of discs with
+    sharp edges (the features ORB finds at MEDIUM resolution) and sensor noise of a few levels on top -- so the FINAL
+    images carry detail down to the pixel.  Only integer arithmetic and +, -, *, /, floor in float64 are used (all
+    correctly rounded), so the views come out byte-identical on any machine, without cv2."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    f = 0.9 * w
+    unit = w / 1000.0  # the shapes of synthetic_views, in units of a 1000 px wide view
+    xs = (np.arange(w, dtype=np.float64) - w / 2) / f
+    band = 256
+    views = []
+
+    def render(img, k, gain, u_row, k_row, y0):
+        ys = (np.arange(y0, min(h, y0 + band), dtype=np.float64) - h / 2) / f
+        u = np.broadcast_to(u_row, (ys.size, w))
+        v = ys[:, None] * k_row[None, :]
+        hb = _mix(np.floor(u / (60 * unit)).astype(np.int64), np.floor(v / (60 * unit)).astype(np.int64), seed)
+        px = np.stack([_byte(hb, 8 * ch, 40, 216) for ch in range(3)], -1)
+        hm = _mix(np.floor(u / (9 * unit)).astype(np.int64), np.floor(v / (9 * unit)).astype(np.int64), seed + 3)
+        px += _byte(hm, 0, -36, 37)[..., None]  # a cell texture that makes every neighbourhood unlike the others
+        _discs(u, v, 120 * unit, 10 * unit, 45 * unit, seed + 1, px)
+        _discs(u, v, 36 * unit, 3 * unit, 12 * unit, seed + 2, px)
+        px += np.random.default_rng([seed, k, y0]).integers(-6, 7, px.shape, dtype=np.int32)
+        img[y0:y0 + ys.size] = np.clip(px * gain // 100, 0, 255).astype(np.uint8)
+
+    with ThreadPoolExecutor(min(8, os.cpu_count() or 1)) as pool:  # bands are independent: any order gives the same bytes
+        for k, (t, gain) in enumerate(zip(CAMERA_VIEW_YAWS[n], CAMERA_VIEW_GAINS[n])):
+            s, c = 2 * t / (1 + t * t), (1 - t * t) / (1 + t * t)
+            den = s * xs + c                                       # ray (x, y, 1) turned by the yaw, divided through by z
+            u_row, k_row = f * (c * xs - s) / den, f / den
+            img = np.empty((h, w, 3), np.uint8)
+            list(pool.map(lambda y0: render(img, k, gain, u_row, k_row, y0), range(0, h, band)))
+            views.append(img)
+    return views
+
+
 PIPELINE_SETTINGS = dict(crop=False, detector="orb", confidence_threshold=0.3)
 
 
