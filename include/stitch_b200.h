@@ -198,13 +198,21 @@ typedef struct {
  * offset or size, an empty slice or a slice larger than its prepared size fails (SB_ERR_INVALID, named in sb_last_error):
  * the reference's blenders cannot feed an empty image either. */
 SB_API sb_compositor *sb_compositor_create_cropped(const sb_rig *rig, const sb_crop *crop, int rank, int world);
+/* sb_compositor_create_cropped (crop may be NULL) taking camera-resolution frames, as Stitcher does when final_megapix is
+ * set: sb_compositor_upload / _submit take image i as in_w[i] x in_h[i], and the library resizes it on the device to its
+ * FINAL size rig->src_w[i] x rig->src_h[i] (what is warped) exactly as Images.resize_img_by_scaler does
+ * (cv.resize INTER_LINEAR_EXACT).  An image whose two sizes are equal is taken as it is.  An input size that is not
+ * positive, smaller than the FINAL size on either axis (the reference never scales up) or with a side of 32767 px or
+ * more fails (SB_ERR_INVALID, the image named in sb_last_error). */
+SB_API sb_compositor *sb_compositor_create_resized(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h,
+                                                   int rank, int world);
 /* geometry of the plan: per image warped rect {x,y,w,h} (== sb_warp_roi; with a crop: feed corner and fed size) and the
  * pano roi {x,y,w,h} */
 SB_API int sb_compositor_geometry(const sb_compositor *c, int *rects /*[n][4]*/, int pano_roi[4], int *num_bands);
 /* compulsory HBM traffic of one run (DESIGN.md byte model) for the roofline: total, and per kernel launch in
  * launch order (same order as sb_compositor_stage_times).  Returns the number of launches (or < 0). */
 SB_API int sb_compositor_model_bytes(const sb_compositor *c, double *total_bytes, double *per_launch, int cap);
-/* host -> device copy of source image i (uint8 HxWx3); asynchronous on the compositor stream when
+/* host -> device copy of source image i (uint8 HxWx3, the input size with sb_compositor_create_resized); asynchronous on the compositor stream when
  * `pinned` != 0 (caller guarantees page-locked memory and keeps it alive until sync) */
 SB_API int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pitch, int pinned);
 /* optional per-image blend mask in warped coordinates (mask_mode 1), uint8 h' x w' */

@@ -96,6 +96,7 @@ SIGNATURES = [
     ("sb_compositor_stage_times", C.c_int, [C.c_void_p, C.POINTER(C.c_char_p), c_float_p, C.c_int]),
     ("sb_compositor_create_sharded", C.c_void_p, [C.POINTER(Rig), C.c_int, C.c_int]),
     ("sb_compositor_create_cropped", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), C.c_int, C.c_int]),
+    ("sb_compositor_create_resized", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), c_int_p, c_int_p, C.c_int, C.c_int]),
     ("sb_compositor_shard_info", C.c_int, [C.c_void_p, c_int_p, c_int_p, c_int_p]),
     ("sb_compositor_shard_phase", C.c_int, [C.c_void_p, C.c_int]),
     ("sb_compositor_shard_slab", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]),

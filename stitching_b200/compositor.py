@@ -63,7 +63,7 @@ class Crop:
 
 class Compositor:
     def __init__(self, cameras, sizes, warper_type="spherical", blender_type="multiband", blend_strength=5, scale=None,
-                 aspect=1, rank=0, world=1, crop=None):
+                 aspect=1, rank=0, world=1, crop=None, input_sizes=None):
         """cameras: objects with .focal, .K(), .R (cv.detail.CameraParams or rigs.Camera); sizes: [(w, h)].
 
         crop: a `Crop` (e.g. Crop.from_cropper(stitcher.cropper, aspect)); every image is then warped only over its
@@ -72,7 +72,13 @@ class Compositor:
 
         world > 1: one panorama over `world` GPUs, one process per GPU.  Every rank passes ALL cameras; rank r owns
         images [r*n/world, (r+1)*n/world) -- `self.first`, `self.count` -- uploads only those and gets the column
-        strip `self.strip` = (lo, hi) of the panorama back (stitching_b200.dist.init_comm must have run)."""
+        strip `self.strip` = (lo, hi) of the panorama back (stitching_b200.dist.init_comm must have run).
+
+        input_sizes: [(w, h)] of the frames upload / submit / composite then take, e.g. the camera sizes `st.images.sizes`
+        of a Stitcher whose final_megapix is set; `sizes` stay the FINAL sizes
+        (`st.images.get_scaled_img_sizes(Images.Resolution.FINAL)`).  Frame i is resized from input_sizes[i] to sizes[i] on
+        the device, byte for byte as Images.resize_img_by_scaler does (cv.resize INTER_LINEAR_EXACT); a frame whose two
+        sizes are equal is taken as it is.  Inputs smaller than their FINAL size on either axis are refused."""
         n = len(cameras)
         if n == 0 or len(sizes) != n:
             raise StitchingError("Compositor needs one size per camera")
@@ -84,6 +90,9 @@ class Compositor:
             raise StitchingError(f"unknown blender type '{blender_type}'")
         self.n = n
         self.sizes = [(int(w), int(h)) for w, h in sizes]
+        if input_sizes is not None and len(input_sizes) != n:
+            raise StitchingError(f"Compositor has {len(input_sizes)} input sizes for {n} images")
+        self.input_sizes = self.sizes if input_sizes is None else [(int(w), int(h)) for w, h in input_sizes]
         if scale is None:
             scale = median([cam.focal for cam in cameras])  # Warper.set_scale
         # Stitcher's ratios are numpy float64, so Warper.get_K scales the float32 K in double and rounds once; a Python
@@ -99,9 +108,16 @@ class Compositor:
                        self._R.ctypes.data_as(_lib.c_float_p), 0)
         L = self._L = _lib.lib()  # close() releases through the library that created the compositor
         self.rank, self.world = int(rank), int(world)
+        desc = None
         if crop is not None:
             arrs = [(C.c_int * (k * n))(*[v for t in ts for v in t]) for k, ts in ((4, crop.rects), (2, crop.corners), (2, crop.sizes))]
             desc = _lib.CropDesc(*[C.cast(a, _lib.c_int_p) for a in arrs])
+        if input_sizes is not None:
+            in_w = (C.c_int * n)(*[s[0] for s in self.input_sizes])
+            in_h = (C.c_int * n)(*[s[1] for s in self.input_sizes])
+            self._c = L.sb_compositor_create_resized(C.byref(rig), C.byref(desc) if desc is not None else None, in_w, in_h,
+                                                     self.rank, self.world)
+        elif crop is not None:
             self._c = L.sb_compositor_create_cropped(C.byref(rig), C.byref(desc), self.rank, self.world)
         elif self.world > 1:
             self._c = L.sb_compositor_create_sharded(C.byref(rig), self.rank, self.world)
@@ -130,8 +146,9 @@ class Compositor:
             raise StitchingError(f"expected {self.count} images (block {self.first}..{self.first + self.count - 1}), got {len(images)}")
         for i, img in enumerate(images, start=self.first):
             img = np.asarray(img)
-            if img.dtype != np.uint8 or img.shape != (self.sizes[i][1], self.sizes[i][0], 3):
-                raise StitchingError(f"image {i}: expected uint8 {self.sizes[i][1]}x{self.sizes[i][0]}x3")
+            w, h = self.input_sizes[i]
+            if img.dtype != np.uint8 or img.shape != (h, w, 3):
+                raise StitchingError(f"image {i}: expected uint8 {h}x{w}x3")
             if img.strides[2] != 1 or img.strides[1] != 3:
                 img = np.ascontiguousarray(img)
             _lib.check(L.sb_compositor_upload(self._c, i, img.ctypes.data_as(C.c_void_p), img.strides[0], int(pinned)),
@@ -219,8 +236,9 @@ class Compositor:
         ptrs = (C.c_void_p * n)()
         pitches = (C.c_size_t * n)()
         for i, img in enumerate(images):
-            if img.dtype != np.uint8 or img.shape != (self.sizes[i][1], self.sizes[i][0], 3) or img.strides[1:] != (3, 1):
-                raise StitchingError(f"image {i}: expected a uint8 {self.sizes[i][1]}x{self.sizes[i][0]}x3 array with packed pixels")
+            w, h = self.input_sizes[i]
+            if img.dtype != np.uint8 or img.shape != (h, w, 3) or img.strides[1:] != (3, 1):
+                raise StitchingError(f"image {i}: expected a uint8 {h}x{w}x3 array with packed pixels")
             ptrs[i] = img.ctypes.data
             pitches[i] = img.strides[0]
         ticket = C.c_ulonglong()

@@ -28,6 +28,9 @@ using namespace sb;
 struct Slot {
     std::vector<uint8_t *> src;    // u8x3 sources as uploaded (null: an image of another rank)
     std::vector<uint32_t *> src4;  // the same, one word per pixel: what the warp kernel reads (repacked after every upload)
+    // An image resized on the device (sb_compositor_create_resized) has its camera-size frame in `src` and its FINAL-size
+    // source, written by k_resize_src, in `src4` when the warp kernel reads words, else in `fin` (packed u8x3).
+    std::vector<uint8_t *> fin;
     PanoOut out{};                 // device outputs
     cudaEvent_t e_h2d = nullptr, e_comp = nullptr, e_d2h = nullptr;  // submit: sources uploaded, step done, output downloaded
 #ifndef SB_EMU
@@ -38,7 +41,11 @@ struct Slot {
 struct sb_compositor {
     int n = 0;
     cudaStream_t stream = nullptr;
-    std::vector<int> src_w, src_h;
+    std::vector<int> src_w, src_h;     // FINAL sizes: what is warped
+    std::vector<int> in_w, in_h;       // the frames upload / submit take: src_w / src_h unless resized on the device
+    std::vector<int *> taps_dev;       // resized images: [x taps | y taps] (resize_exact_taps), null for the others
+    std::vector<char> warp_src4;       // resized images: the warp kernel reads the word-per-pixel source
+    std::vector<ResizeJob> resize_jobs;  // scratch of prepare_sources
     std::vector<Rect> rects;           // warped rects (pano-absolute)
     std::vector<WarpJob> jobs;         // host copy, reading slot 0's sources
     std::vector<WarpJob> slot_jobs;    // scratch: the jobs of another slot (slot_jobs_of)
@@ -77,8 +84,17 @@ static int slot_alloc(sb_compositor *c, Slot &sl)
     cudaStream_t s = c->stream;
     sl.src.assign(c->n, nullptr);
     sl.src4.assign(c->n, nullptr);
+    sl.fin.assign(c->n, nullptr);
     for (int i = c->first; i < c->first + c->count; ++i) {
         const long long px = (long long)c->src_w[i] * c->src_h[i];
+        if (c->taps_dev[i]) {
+            SB_TRY(dev_alloc((void **)&sl.src[i], (size_t)c->in_w[i] * c->in_h[i] * 3 + SB_SRC_PAD, s));
+            if (c->warp_src4[i])
+                SB_TRY(dev_alloc((void **)&sl.src4[i], ((size_t)px + 4) * sizeof(uint32_t), s));
+            else
+                SB_TRY(dev_alloc((void **)&sl.fin[i], (size_t)px * 3 + SB_SRC_PAD, s));
+            continue;
+        }
         SB_TRY(dev_alloc((void **)&sl.src[i], (size_t)px * 3 + SB_SRC_PAD, s));
         if (c->use_src4 && px < (1ll << 31)) SB_TRY(dev_alloc((void **)&sl.src4[i], ((size_t)px + 4) * sizeof(uint32_t), s));
     }
@@ -99,6 +115,7 @@ static void slot_free(Slot &sl, cudaStream_t s)
 {
     for (auto p : sl.src) dev_free(p, s);
     for (auto p : sl.src4) dev_free(p, s);
+    for (auto p : sl.fin) dev_free(p, s);
     dev_free(sl.out.rgb, s);
     dev_free(sl.out.mask, s);
     for (cudaEvent_t e : {sl.e_h2d, sl.e_comp, sl.e_d2h})
@@ -119,6 +136,7 @@ static void compositor_free(sb_compositor *c)
     for (auto p : c->tab_dev) dev_free(p, s);
     for (auto p : c->maps_dev) dev_free(p, s);
     for (auto p : c->usermask_dev) dev_free(p, s);
+    for (auto p : c->taps_dev) dev_free(p, s);
     for (auto &g : c->gain) gain_free(&g, s);
     dev_free(c->flush_buf, s);
     if (c->h2d) (void)cudaStreamDestroy(c->h2d);
@@ -169,7 +187,84 @@ static int crop_image(const sb_crop *crop, int i, const Rect &warped, Rect *proj
     return SB_OK;
 }
 
-static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *crop, int rank, int world)
+// the packed source the warp kernel of image i reads in `sl` (the FINAL-size one of a resized image)
+static const uint8_t *warp_src(const sb_compositor *c, const Slot &sl, int i) { return c->taps_dev[i] ? sl.fin[i] : sl.src[i]; }
+
+// Images.resize_img_by_scaler sizes: the reference resizes camera frames to the FINAL sizes with cv.resize and never
+// scales up (MegapixDownscaler); the staging buffers hold the frames, so they obey the compositor's source limit
+static int check_input_sizes(const sb_rig *rig, const int *in_w, const int *in_h)
+{
+    for (int i = 0; i < rig->n_images; ++i) {
+        const int w = in_w[i], h = in_h[i], fw = rig->src_w[i], fh = rig->src_h[i];
+        if (w <= 0 || h <= 0) {
+            set_error("compositor: input frame of image %d has the size %dx%d", i, w, h);
+            return SB_ERR_INVALID;
+        }
+        if (w >= SB_MAX_WARP_SIDE || h >= SB_MAX_WARP_SIDE) {
+            set_error("compositor: input frame of image %d (%dx%d) has a side of %d px or more", i, w, h, SB_MAX_WARP_SIDE);
+            return SB_ERR_INVALID;
+        }
+        if (w < fw || h < fh) {
+            set_error("compositor: input frame of image %d (%dx%d) is smaller than its FINAL size %dx%d on some axis; frames are "
+                      "only scaled down", i, w, h, fw, fh);
+            return SB_ERR_INVALID;
+        }
+    }
+    return SB_OK;
+}
+
+// The taps of the resized images of this rank, and which source layout their warp kernel reads: launch_warp chooses
+// its kernel per batch of SB_WARP_BATCH jobs, and reads the word-per-pixel sources only when the RGBM kernel runs and
+// every job of the batch has one (slot_alloc's rule); a resized image gets only the buffer that is read.
+static int plan_resize(sb_compositor *c, cudaStream_t s)
+{
+    std::vector<int> t;
+    for (int b = c->first; b < c->first + c->count; b += SB_WARP_BATCH) {
+        const int end = std::min(b + SB_WARP_BATCH, c->first + c->count);
+        bool words = warp_batch_rgbm(c->jobs.data() + b, end - b);
+        for (int i = b; i < end; ++i) words = words && c->use_src4 && (long long)c->src_w[i] * c->src_h[i] < (1ll << 31);
+        for (int i = b; i < end; ++i) {
+            const int w = c->src_w[i], h = c->src_h[i];
+            if (c->in_w[i] == w && c->in_h[i] == h) continue;
+            c->warp_src4[i] = words;
+            t.resize((size_t)3 * (w + h));
+            resize_exact_taps(c->in_w[i], w, t.data());
+            resize_exact_taps(c->in_h[i], h, t.data() + (size_t)3 * w);
+            SB_TRY(dev_alloc((void **)&c->taps_dev[i], t.size() * sizeof(int), s));
+            SB_CUDA(cudaMemcpyAsync(c->taps_dev[i], t.data(), t.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+            SB_CUDA(cudaStreamSynchronize(s));  // t is reused by the next image
+        }
+    }
+    return SB_OK;
+}
+
+// After the frames of images [i0, i1) have reached `sl.src` (in the order of stream s): the sources the warp kernel
+// reads -- the repack, or for a resized image k_resize_src in its place, one launch for all of them
+static int prepare_sources(sb_compositor *c, const Slot &sl, int i0, int i1, cudaStream_t s)
+{
+    c->resize_jobs.clear();
+    for (int i = i0; i < i1; ++i) {
+        if (c->taps_dev[i]) {
+            ResizeJob r;
+            r.src = sl.src[i];
+            r.dst4 = sl.src4[i];
+            r.dst3 = sl.fin[i];
+            r.tx = c->taps_dev[i];
+            r.ty = c->taps_dev[i] + (size_t)3 * c->src_w[i];
+            r.sw = c->in_w[i];
+            r.dw = c->src_w[i];
+            r.px = (long long)c->src_w[i] * c->src_h[i];
+            c->resize_jobs.push_back(r);
+        } else if (sl.src4[i]) {
+            SB_TRY(launch_repack_rgbx(sl.src[i], sl.src4[i], (long long)c->src_w[i] * c->src_h[i], s));
+        }
+    }
+    return c->resize_jobs.empty() ? SB_OK : launch_resize_src(c->resize_jobs.data(), (int)c->resize_jobs.size(), s);
+}
+
+// in_w / in_h: null, or the size of the frame of every image (sb_compositor_create_resized)
+static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h, int rank,
+                            int world)
 {
     const int n = rig->n_images;
     c->n = n;
@@ -184,6 +279,11 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *
 
     c->src_w.assign(rig->src_w, rig->src_w + n);
     c->src_h.assign(rig->src_h, rig->src_h + n);
+    if (in_w) SB_TRY(check_input_sizes(rig, in_w, in_h));
+    c->in_w.assign(in_w ? in_w : rig->src_w, (in_w ? in_w : rig->src_w) + n);
+    c->in_h.assign(in_h ? in_h : rig->src_h, (in_h ? in_h : rig->src_h) + n);
+    c->taps_dev.assign(n, nullptr);
+    c->warp_src4.assign(n, 0);
     c->rects.resize(n);
     c->jobs.resize(n);
     {
@@ -282,12 +382,13 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *
     }
     SB_TRY(c->plan.allocate(s));
     if (c->sharded) SB_TRY(c->shard.allocate(c->plan, s));
+    SB_TRY(plan_resize(c, s));
     c->slots[0].out.w = out_w;
     c->slots[0].out.h = out_h;
     SB_TRY(slot_alloc(c, c->slots[0]));
     c->n_slots = 1;
     for (int i = c->first; i < c->first + c->count; ++i) {
-        c->jobs[i].src = c->slots[0].src[i];
+        c->jobs[i].src = warp_src(c, c->slots[0], i);
         c->jobs[i].src4 = c->slots[0].src4[i];
     }
     SB_CUDA(cudaStreamSynchronize(s));
@@ -300,7 +401,7 @@ static const WarpJob *slot_jobs_of(sb_compositor *c, int slot)
     if (slot == 0) return c->jobs.data();
     c->slot_jobs = c->jobs;
     for (int i = 0; i < c->n; ++i) {
-        c->slot_jobs[i].src = c->slots[slot].src[i];
+        c->slot_jobs[i].src = warp_src(c, c->slots[slot], i);
         c->slot_jobs[i].src4 = c->slots[slot].src4[i];
     }
     return c->slot_jobs.data();
@@ -564,10 +665,11 @@ static bool valid_rig(const sb_rig *rig)
            rig->blend_kind <= SB_BLEND_MULTIBAND;
 }
 
-static sb_compositor *compositor_create(const sb_rig *rig, const sb_crop *crop, int rank, int world)
+static sb_compositor *compositor_create(const sb_rig *rig, const sb_crop *crop, int rank, int world, const int *in_w = nullptr,
+                                        const int *in_h = nullptr)
 {
     sb_compositor *c = new sb_compositor;
-    if (compositor_build(c, rig, crop, rank, world) != SB_OK) {
+    if (compositor_build(c, rig, crop, in_w, in_h, rank, world) != SB_OK) {
         compositor_free(c);
         return nullptr;
     }
@@ -604,6 +706,18 @@ sb_compositor *sb_compositor_create_cropped(const sb_rig *rig, const sb_crop *cr
         return nullptr;
     }
     return compositor_create(rig, crop, rank, world);
+}
+
+// Any of the above taking camera-size frames: image i is uploaded / submitted at in_w[i] x in_h[i] and resized on the
+// device to its FINAL size rig->src_w[i] x rig->src_h[i] (Images.resize_img_by_scaler), or taken as it is when the two
+// sizes are equal
+sb_compositor *sb_compositor_create_resized(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h, int rank, int world)
+{
+    if (!valid_rig(rig) || !in_w || !in_h || world < 1 || rank < 0 || rank >= world || (crop && (!crop->rect || !crop->corner || !crop->size))) {
+        set_error("sb_compositor_create_resized: invalid argument");
+        return nullptr;
+    }
+    return compositor_create(rig, crop, rank, world, in_w, in_h);
 }
 
 int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_local, int strip[2])
@@ -702,7 +816,7 @@ int sb_compositor_model_bytes(const sb_compositor *c, double *total_bytes, doubl
 
 int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pitch, int pinned)
 {
-    if (!c || i < 0 || i >= c->n || !src || pitch < (size_t)c->src_w[i] * 3) {
+    if (!c || i < 0 || i >= c->n || !src || pitch < (size_t)c->in_w[i] * 3) {
         set_error("sb_compositor_upload: invalid argument");
         return SB_ERR_INVALID;
     }
@@ -711,9 +825,9 @@ int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pit
         set_error("sb_compositor_upload: image %d belongs to another rank (this rank owns %d..%d)", i, c->first, c->first + c->count - 1);
         return SB_ERR_INVALID;
     }
-    SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->src_w[i] * 3, src, pitch, (size_t)c->src_w[i] * 3, c->src_h[i],
-                              cudaMemcpyHostToDevice, c->stream));
-    if (sl.src4[i]) SB_TRY(launch_repack_rgbx(sl.src[i], sl.src4[i], (long long)c->src_w[i] * c->src_h[i], c->stream));
+    SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->in_w[i] * 3, src, pitch, (size_t)c->in_w[i] * 3, c->in_h[i], cudaMemcpyHostToDevice,
+                      c->stream));
+    SB_TRY(prepare_sources(c, sl, i, i + 1, c->stream));
     if (!pinned) SB_CUDA(cudaStreamSynchronize(c->stream));
     return SB_OK;
 }
@@ -805,7 +919,7 @@ int sb_compositor_submit(sb_compositor *c, const uint8_t *const *srcs, const siz
         return SB_ERR_STATE;
     }
     for (int i = 0; i < c->n; ++i)
-        if (!srcs[i] || pitches[i] < (size_t)c->src_w[i] * 3) {
+        if (!srcs[i] || pitches[i] < (size_t)c->in_w[i] * 3) {
             set_error("sb_compositor_submit: invalid source %d", i);
             return SB_ERR_INVALID;
         }
@@ -819,12 +933,11 @@ int sb_compositor_submit(sb_compositor *c, const uint8_t *const *srcs, const siz
     if (t < SB_PIPE_DEPTH) SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
     SB_CUDA(cudaStreamWaitEvent(c->h2d, sl.e_comp, 0));
     for (int i = 0; i < c->n; ++i)
-        SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->src_w[i] * 3, srcs[i], pitches[i], (size_t)c->src_w[i] * 3, c->src_h[i],
+        SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->in_w[i] * 3, srcs[i], pitches[i], (size_t)c->in_w[i] * 3, c->in_h[i],
                                   cudaMemcpyHostToDevice, c->h2d));
-    // the repack kernels follow the LAST copy (same stream): a kernel between two copies would leave the PCIe link idle
-    // for its launch + run time, eight times per step
-    for (int i = 0; i < c->n; ++i)
-        if (sl.src4[i]) SB_TRY(launch_repack_rgbx(sl.src[i], sl.src4[i], (long long)c->src_w[i] * c->src_h[i], c->h2d));
+    // the repack (and resize) kernels follow the LAST copy (same stream): a kernel between two copies would leave the PCIe
+    // link idle for its launch + run time, eight times per step
+    SB_TRY(prepare_sources(c, sl, 0, c->n, c->h2d));
     SB_CUDA(cudaEventRecord(sl.e_h2d, c->h2d));
     SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_h2d, 0));
     // the output buffers of this slot are free once their previous download has finished

@@ -217,6 +217,22 @@ int launch_warp(const WarpJob *jobs_host, int n_jobs, cudaStream_t s);
 int warp_maps_upload(const Projector &p, const int rect[4], float *maps_dev, WarpJob *job, cudaStream_t s);  // sb_api.cpp
 // u8x3 contiguous (w * h pixels) -> r | g<<8 | b<<16 words (the compositor's source layout for the warp kernel)
 int launch_repack_rgbx(const uint8_t *rgb, uint32_t *dst, long long pixels, cudaStream_t s);
+// launch_warp's kernel choice for a batch of jobs: true when it reads WarpJob::src4 of jobs that have one (sb_warp.cu)
+bool warp_batch_rgbm(const WarpJob *jobs, int cnt);
+// one image of k_resize_src: Images.resize_img_by_scaler (cv.resize INTER_LINEAR_EXACT) from a camera-size frame into
+// the warp's source layout, in place of the repack (sb_compositor_create_resized)
+struct ResizeJob {
+    const uint8_t *src;  // camera-size u8x3, rows of 3 * sw bytes, SB_SRC_PAD spare bytes after the last
+    uint32_t *dst4;      // FINAL size, one word per pixel (WarpJob::src4), or null:
+    uint8_t *dst3;       //   then FINAL size, packed u8x3 (WarpJob::src)
+    const int *tx, *ty;  // device taps [i0 | i1 | c1] of the two axes (resize_exact_taps), dw / dh entries each
+    int sw, dw;
+    long long px;        // dw * dh
+};
+struct ResizeBatch {
+    ResizeJob j[SB_WARP_BATCH];
+};
+int launch_resize_src(const ResizeJob *jobs, int n_jobs, cudaStream_t s);  // one launch per SB_WARP_BATCH images
 int launch_pack_rgbm(const uint8_t *rgb, long long rgb_pitch, const uint8_t *mask, long long mask_pitch, uint32_t *dst,
                      long long dst_pitch, int w, int h, cudaStream_t s);
 // level `l` -> `l+1` of images [first, first+count)

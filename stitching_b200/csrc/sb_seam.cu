@@ -51,19 +51,18 @@ __global__ void k_resize_linear_and(const uint8_t *__restrict__ src, int sw, con
 }
 
 // cv.resize(uint8, cn channels, INTER_LINEAR_EXACT) (Images.resize_img_by_scaler, stitching/images.py:120-123): OpenCV's
-// bit-exact 8.8 / 16.16 fixed-point bilinear; taps [i0 | i1 | c1] per axis from the host (resize_exact_taps)
+// bit-exact 8.8 / 16.16 fixed-point bilinear (resize_exact_value); taps [i0 | i1 | c1] per axis from the host
+// (resize_exact_taps)
 __global__ void k_resize_exact(const uint8_t *__restrict__ src, long long spitch, int cn, const int *__restrict__ tx,
                                const int *__restrict__ ty, uint8_t *__restrict__ dst, long long dpitch, int w, int h)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= w || y >= h) return;
-    const unsigned cx1 = (unsigned)tx[2 * w + x], cx0 = 256u - cx1, cy1 = (unsigned)ty[2 * h + y], cy0 = 256u - cy1;
+    const unsigned cx1 = (unsigned)tx[2 * w + x], cy1 = (unsigned)ty[2 * h + y];
     const uint8_t *r0 = src + ty[y] * spitch, *r1 = src + ty[h + y] * spitch;
     const int x0 = tx[x] * cn, x1 = tx[w + x] * cn;
-    for (int c = 0; c < cn; ++c) {
-        const unsigned h0 = r0[x0 + c] * cx0 + r0[x1 + c] * cx1, h1 = r1[x0 + c] * cx0 + r1[x1 + c] * cx1;  // 8.8
-        dst[y * dpitch + (long long)x * cn + c] = (uint8_t)((h0 * cy0 + h1 * cy1 + (1u << 15)) >> 16);
-    }
+    for (int c = 0; c < cn; ++c)
+        dst[y * dpitch + (long long)x * cn + c] = (uint8_t)resize_exact_value(r0[x0 + c], r0[x1 + c], r1[x0 + c], r1[x1 + c], cx1, cy1);
 }
 
 }  // namespace

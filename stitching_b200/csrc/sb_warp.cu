@@ -420,6 +420,59 @@ __global__ void __launch_bounds__(256) k_repack_rgbx(const uint8_t *__restrict__
     }
 }
 
+// Images.resize_img_by_scaler (cv.resize INTER_LINEAR_EXACT, resize_exact_rgb) from a camera-size u8x3 frame straight
+// into the warp's source layout, in place of k_repack_rgbx.  Thread t of image blockIdx.z computes the FINAL pixels
+// 4t .. 4t+3 in row-major order (a group may wrap into the next row), so that the word layout gets one aligned 16-byte
+// store per thread and the packed one three aligned words: neither FINAL layout has row padding (the warp kernel indexes
+// them by width), and a group of four is the largest that stays aligned for any width.  A warp covers 128 consecutive
+// pixels of (mostly) one row; the two source rows each reads are 6-byte pairs fetched with aligned 8-byte loads
+// (fetch_pair: the staging buffer has SB_SRC_PAD spare bytes).  At scales >= 0.5 consecutive FINAL rows share source
+// rows, and the blocks of one FINAL row are launched next to those of the following one, so the second reader finds the
+// row in L2: the frame crosses HBM about once.
+__global__ void __launch_bounds__(256) k_resize_src(const __grid_constant__ ResizeBatch B)
+{
+    const ResizeJob &j = B.j[blockIdx.z];
+    const long long p = 4 * ((long long)blockIdx.x * blockDim.x + threadIdx.x);
+    if (p >= j.px) return;
+    const int np = j.px - p < 4 ? (int)(j.px - p) : 4;
+    int y = (int)(p / j.dw), x = (int)(p - (long long)y * j.dw);
+    const int dh = (int)(j.px / j.dw);
+    const unsigned pitch = 3u * (unsigned)j.sw;  // sides < 32767: row offsets stay below 2^32
+    unsigned out[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        if (k < np) {
+            const int x0 = __ldg(j.tx + x), x1 = __ldg(j.tx + j.dw + x);
+            unsigned a0, a1, b0, b1;
+            fetch_pair(j.src, (unsigned)__ldg(j.ty + y) * pitch, x0, x1, a0, a1);
+            fetch_pair(j.src, (unsigned)__ldg(j.ty + dh + y) * pitch, x0, x1, b0, b1);
+            out[k] = resize_exact_rgb(a0, a1, b0, b1, (unsigned)__ldg(j.tx + 2 * j.dw + x), (unsigned)__ldg(j.ty + 2 * dh + y));
+        }
+        if (++x == j.dw) {
+            x = 0;
+            ++y;
+        }
+    }
+    if (j.dst4) {
+        if (np == 4)
+            *reinterpret_cast<uint4 *>(j.dst4 + p) = make_uint4(out[0], out[1], out[2], out[3]);  // the allocator aligns to 256 bytes
+        else
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                if (k < np) j.dst4[p + k] = out[k];
+    } else if (np == 4) {  // 12 bytes at a multiple of 12: three aligned words
+        unsigned *d = reinterpret_cast<unsigned *>(j.dst3 + 3 * p);
+        d[0] = out[0] | (out[1] << 24);
+        d[1] = (out[1] >> 8) | (out[2] << 16);
+        d[2] = (out[2] >> 16) | (out[3] << 8);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            if (k < np)
+                for (int c = 0; c < 3; ++c) j.dst3[3 * (p + k) + c] = (uint8_t)(out[k] >> (8 * c));
+    }
+}
+
 __global__ void k_pack_rgbm(const uint8_t *__restrict__ rgb, long long rgb_pitch, const uint8_t *__restrict__ mask,
                             long long mask_pitch, uint32_t *__restrict__ dst, long long dst_pitch, int w, int h)
 {
@@ -441,6 +494,36 @@ int launch_repack_rgbx(const uint8_t *rgb, uint32_t *dst, long long pixels, cuda
     return launch_check("k_repack_rgbx");
 }
 
+int launch_resize_src(const ResizeJob *jobs, int n_jobs, cudaStream_t s)
+{
+    for (int first = 0; first < n_jobs; first += SB_WARP_BATCH) {
+        const int cnt = n_jobs - first < SB_WARP_BATCH ? n_jobs - first : SB_WARP_BATCH;
+        ResizeBatch B;
+        long long max_px = 0;
+        for (int i = 0; i < cnt; ++i) {
+            B.j[i] = jobs[first + i];
+            max_px = max_px > B.j[i].px ? max_px : B.j[i].px;
+        }
+        for (int i = cnt; i < SB_WARP_BATCH; ++i) B.j[i] = B.j[0];
+        const long long threads = (max_px + 3) / 4;
+        launch(k_resize_src, dim3((unsigned)((threads + 255) / 256), 1, cnt), dim3(256), 0, s, B);
+        SB_TRY(launch_check("k_resize_src"));
+    }
+    return SB_OK;
+}
+
+// launch_warp's kernel for a batch: the RGBM kernel from separable tables when every job qualifies, else k_warp_wide
+// (or k_warp_gather under SB_KERNELS=simple); only the RGBM kernel reads word-per-pixel sources
+bool warp_batch_rgbm(const WarpJob *j, int cnt)
+{
+    if (use_simple_kernels()) return false;
+    for (int i = 0; i < cnt; ++i)
+        if (j[i].xmap || !j[i].dst_rgbm || j[i].dst_rgb || j[i].dst_mask || j[i].sw > 32767 || j[i].sh > 32767 || j[i].sw < 2 ||
+            j[i].sh < 2 || j[i].rgbm_pitch % 2 != 0)
+            return false;
+    return true;
+}
+
 int launch_warp(const WarpJob *jobs_host, int n_jobs, cudaStream_t s)
 {
     for (int first = 0; first < n_jobs; first += SB_WARP_BATCH) {
@@ -456,14 +539,12 @@ int launch_warp(const WarpJob *jobs_host, int n_jobs, cudaStream_t s)
         if (max_w <= 0 || max_h <= 0) continue;
         dim3 block(WARP_BX, WARP_BY), grid(div_up(max_w, WARP_BX), div_up(max_h, WARP_BY), cnt);
         if (!use_simple_kernels()) {
-            bool rgbm_only = true, has_bm = false, src4 = true;
+            bool has_bm = false, src4 = true;
             for (int i = 0; i < cnt; ++i) {
                 src4 = src4 && B.j[i].src4 != nullptr;
-                rgbm_only = rgbm_only && !B.j[i].xmap && B.j[i].dst_rgbm && !B.j[i].dst_rgb && !B.j[i].dst_mask && B.j[i].sw <= 32767 && B.j[i].sh <= 32767 &&
-                            B.j[i].sw >= 2 && B.j[i].sh >= 2 && B.j[i].rgbm_pitch % 2 == 0;
                 has_bm = has_bm || B.j[i].blend_mask || B.j[i].gain_mode;  // per-pixel extras anywhere in the batch
             }
-            if (rgbm_only) {
+            if (warp_batch_rgbm(B.j, cnt)) {
                 dim3 grid2(div_up(max_w, 2 * WARP_BX), div_up(max_h, WARP_BY), cnt);
                 if (has_bm && src4)
                     launch_pdl(k_warp_rgbm<true, true, true>, grid2, block, 0, s, B);
