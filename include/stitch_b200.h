@@ -206,6 +206,28 @@ SB_API sb_compositor *sb_compositor_create_cropped(const sb_rig *rig, const sb_c
  * more fails (SB_ERR_INVALID, the image named in sb_last_error). */
 SB_API sb_compositor *sb_compositor_create_resized(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h,
                                                    int rank, int world);
+/* Stitcher with timelapse="as_is" / "crop" (stitcher.py:241-252, timelapser.py): instead of a panorama, every step writes
+ * one frame per image -- cv.detail.Timelapser's canvas, zero except for the fed image i (warped, cropped and compensated)
+ * pasted at its corner.  The canvas is resultRoi (AS_IS) or resultRoiIntersection (CROP, an empty intersection giving the
+ * gap between the images) of what Blender.prepare would have received.  crop, in_w / in_h (both nullable) as in
+ * sb_compositor_create_resized; one GPU; rig->blend_* are unused.  A canvas with a zero side, which the reference's
+ * get_frame cannot show, fails (SB_ERR_INVALID).  sb_compositor_geometry returns the fed rects, the canvas as pano_roi and
+ * num_bands = -1; set_gain, wait, sync, time, stage_times and model_bytes work; upload, run, download, download_warped,
+ * submit, set_mask, set_seam_mask, time_multi and the shard hooks fail with SB_ERR_STATE. */
+typedef enum { SB_TIMELAPSE_AS_IS = 1, SB_TIMELAPSE_CROP = 2 } sb_timelapse_kind;
+SB_API sb_compositor *sb_compositor_create_timelapse(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h,
+                                                     int kind);
+/* Pipelined timelapse step: like sb_compositor_submit, but the step ends in the library's frames.  The library owns
+ * 3 x n frames of the canvas in page-locked memory (3 * n * canvas_w * canvas_h * 3 bytes, allocated and zeroed on the first
+ * call; SB_ERR_NOMEM names the byte count when they cannot be had, and the next call tries again); only the part of each
+ * image on the canvas crosses PCIe. */
+SB_API int sb_compositor_submit_timelapse(sb_compositor *c, const uint8_t *const *srcs, const size_t *pitches,
+                                          unsigned long long *ticket);
+/* frame i (uint8 canvas_h x canvas_w x 3, row pitch in bytes) of `ticket`: read it after sb_compositor_wait(ticket); it
+ * stays valid until ticket + 3 is submitted.  Read-only: the library writes only the image's part of it and relies on the
+ * rest staying zero. */
+SB_API int sb_compositor_timelapse_frame(const sb_compositor *c, unsigned long long ticket, int i, const uint8_t **frame,
+                                         size_t *pitch);
 /* geometry of the plan: per image warped rect {x,y,w,h} (== sb_warp_roi; with a crop: feed corner and fed size) and the
  * pano roi {x,y,w,h} */
 SB_API int sb_compositor_geometry(const sb_compositor *c, int *rects /*[n][4]*/, int pano_roi[4], int *num_bands);

@@ -21,6 +21,7 @@ WARP_TYPES = {  # warper.py:10-27 -> sb_warp_type
     "mercator": 14, "transverseMercator": 15,
 }
 BLEND_KINDS = {"no": 0, "feather": 1, "multiband": 2}
+TIMELAPSE_KINDS = {"as_is": 1, "crop": 2}  # timelapser.py:8 -> sb_timelapse_kind
 
 c_float_p = C.POINTER(C.c_float)
 c_int_p = C.POINTER(C.c_int)
@@ -97,6 +98,9 @@ SIGNATURES = [
     ("sb_compositor_create_sharded", C.c_void_p, [C.POINTER(Rig), C.c_int, C.c_int]),
     ("sb_compositor_create_cropped", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), C.c_int, C.c_int]),
     ("sb_compositor_create_resized", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), c_int_p, c_int_p, C.c_int, C.c_int]),
+    ("sb_compositor_create_timelapse", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), c_int_p, c_int_p, C.c_int]),
+    ("sb_compositor_submit_timelapse", C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(C.c_ulonglong)]),
+    ("sb_compositor_timelapse_frame", C.c_int, [C.c_void_p, C.c_ulonglong, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]),
     ("sb_compositor_shard_info", C.c_int, [C.c_void_p, c_int_p, c_int_p, c_int_p]),
     ("sb_compositor_shard_phase", C.c_int, [C.c_void_p, C.c_int]),
     ("sb_compositor_shard_slab", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]),

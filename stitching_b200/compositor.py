@@ -63,7 +63,7 @@ class Crop:
 
 class Compositor:
     def __init__(self, cameras, sizes, warper_type="spherical", blender_type="multiband", blend_strength=5, scale=None,
-                 aspect=1, rank=0, world=1, crop=None, input_sizes=None):
+                 aspect=1, rank=0, world=1, crop=None, input_sizes=None, timelapse=None):
         """cameras: objects with .focal, .K(), .R (cv.detail.CameraParams or rigs.Camera); sizes: [(w, h)].
 
         crop: a `Crop` (e.g. Crop.from_cropper(stitcher.cropper, aspect)); every image is then warped only over its
@@ -78,10 +78,19 @@ class Compositor:
         of a Stitcher whose final_megapix is set; `sizes` stay the FINAL sizes
         (`st.images.get_scaled_img_sizes(Images.Resolution.FINAL)`).  Frame i is resized from input_sizes[i] to sizes[i] on
         the device, byte for byte as Images.resize_img_by_scaler does (cv.resize INTER_LINEAR_EXACT); a frame whose two
-        sizes are equal is taken as it is.  Inputs smaller than their FINAL size on either axis are refused."""
+        sizes are equal is taken as it is.  Inputs smaller than their FINAL size on either axis are refused.
+
+        timelapse: "as_is" or "crop" -- a Stitcher with that timelapse setting: every step ends in one frame per image
+        (Timelapser.process_frame / get_frame) instead of a panorama.  `self.roi` is then the canvas; submit_timelapse /
+        wait / frames, or timelapse(), run the steps; set_gain works, the blend, mask and panorama calls do not.  One GPU
+        only; blender_type and blend_strength are unused."""
         n = len(cameras)
         if n == 0 or len(sizes) != n:
             raise StitchingError("Compositor needs one size per camera")
+        if timelapse is not None and timelapse not in _lib.TIMELAPSE_KINDS:
+            raise StitchingError(f"unknown timelapse kind '{timelapse}' (the compositor writes frames for 'as_is' and 'crop')")
+        if timelapse is not None and int(world) != 1:
+            raise StitchingError("a timelapse compositor runs on one GPU")
         if crop is not None and len(crop.rects) != n:
             raise StitchingError(f"Crop has {len(crop.rects)} rects for {n} images")
         if warper_type not in _lib.WARP_TYPES:
@@ -112,7 +121,13 @@ class Compositor:
         if crop is not None:
             arrs = [(C.c_int * (k * n))(*[v for t in ts for v in t]) for k, ts in ((4, crop.rects), (2, crop.corners), (2, crop.sizes))]
             desc = _lib.CropDesc(*[C.cast(a, _lib.c_int_p) for a in arrs])
-        if input_sizes is not None:
+        self.timelapse_kind = timelapse
+        if timelapse is not None:
+            in_w = (C.c_int * n)(*[s[0] for s in self.input_sizes]) if input_sizes is not None else None
+            in_h = (C.c_int * n)(*[s[1] for s in self.input_sizes]) if input_sizes is not None else None
+            self._c = L.sb_compositor_create_timelapse(C.byref(rig), C.byref(desc) if desc is not None else None, in_w, in_h,
+                                                       _lib.TIMELAPSE_KINDS[timelapse])
+        elif input_sizes is not None:
             in_w = (C.c_int * n)(*[s[0] for s in self.input_sizes])
             in_h = (C.c_int * n)(*[s[1] for s in self.input_sizes])
             self._c = L.sb_compositor_create_resized(C.byref(rig), C.byref(desc) if desc is not None else None, in_w, in_h,
@@ -250,8 +265,57 @@ class Compositor:
     def wait(self, ticket):
         _lib.check(_lib.lib().sb_compositor_wait(self._c, C.c_ulonglong(ticket)), "sb_compositor_wait")
 
+    # -- timelapse (Compositor(..., timelapse="as_is" | "crop")) -------------------------------------------------------
+    def _sources(self, images):
+        if len(images) != self.n:
+            raise StitchingError(f"expected {self.n} images, got {len(images)}")
+        ptrs = (C.c_void_p * self.n)()
+        pitches = (C.c_size_t * self.n)()
+        for i, img in enumerate(images):
+            w, h = self.input_sizes[i]
+            if img.dtype != np.uint8 or img.shape != (h, w, 3) or img.strides[1:] != (3, 1):
+                raise StitchingError(f"image {i}: expected a uint8 {h}x{w}x3 array with packed pixels")
+            ptrs[i] = img.ctypes.data
+            pitches[i] = img.strides[0]
+        return ptrs, pitches
+
+    def submit_timelapse(self, images):
+        """Pipelined timelapse step: enqueue upload of `images`, warp, and the copy of every image's part into its frame;
+        returns a ticket for wait() and frames().  At most three tickets in flight; host arrays should live in pinned
+        memory (`pinned_empty`) and must stay untouched until wait(ticket) returns."""
+        ptrs, pitches = self._sources(images)
+        ticket = C.c_ulonglong()
+        _lib.check(_lib.lib().sb_compositor_submit_timelapse(self._c, ptrs, pitches, C.byref(ticket)), "sb_compositor_submit_timelapse")
+        return ticket.value
+
+    def frames(self, ticket):
+        """The n frames of `ticket` after wait(ticket): read-only uint8 views (canvas h x w x 3) into the library's
+        page-locked frames, valid until ticket + 3 is submitted or close() is called (copy what must live longer).  A
+        view keeps the compositor alive, so dropping the compositor does not free the memory under it; an explicit
+        close() does."""
+        out = []
+        for i in range(self.n):
+            p, pitch = C.c_void_p(), C.c_size_t()
+            _lib.check(_lib.lib().sb_compositor_timelapse_frame(self._c, C.c_ulonglong(ticket), i, C.byref(p), C.byref(pitch)),
+                       "sb_compositor_timelapse_frame")
+            w, h = self.roi[2], self.roi[3]
+            buf = (C.c_uint8 * (pitch.value * h)).from_address(p.value)
+            buf.owner = self  # the ndarray's base is `buf`
+            a = np.ndarray((h, w, 3), np.uint8, buffer=buf, strides=(pitch.value, 3, 1))
+            a.flags.writeable = False
+            out.append(a)
+        return out
+
+    def timelapse(self, images):
+        """One timelapse step: submit_timelapse + wait; returns n owned copies of the frames, as Timelapser.get_frame
+        returns them after process_frame of each image."""
+        images = [np.ascontiguousarray(img) for img in images]
+        t = self.submit_timelapse(images)
+        self.wait(t)
+        return [f.copy() for f in self.frames(t)]
+
     def pinned_empty(self, shape):
-        """uint8 ndarray in page-locked host memory (freed with the compositor)."""
+        """uint8 ndarray in page-locked host memory (freed with the compositor: invalid after close())."""
         nbytes = int(np.prod(shape))
         p = self._L.sb_host_alloc(nbytes)
         if not p:

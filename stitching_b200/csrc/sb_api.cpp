@@ -297,7 +297,7 @@ void gain_free(GainData *gd, cudaStream_t s)
 // ExposureErrorCompensator.apply's per-image data on the device: either the float32 gain map (gc = 1 or 3 channels) with
 // the resize taps for a w x h image, or the three 256-entry tables of scalar gains
 int gain_upload(WarpJob *job, GainData *gd, int w, int h, const float *gain_map, int gw, int gh, int gc, const double *gain_scalar,
-                cudaStream_t s)
+                cudaStream_t s, const int *sub)
 {
     gain_free(gd, s);
     job->gain_mode = 0;
@@ -316,6 +316,20 @@ int gain_upload(WarpJob *job, GainData *gd, int w, int h, const float *gain_map,
     std::vector<float> fx((size_t)w), fy((size_t)h);
     resize_f32_taps(gw, w, tx.data(), fx.data());
     resize_f32_taps(gh, h, ty.data(), fy.data());
+    if (sub) {
+        // the taps of columns [x, x + w') and rows [y, y + h') of the whole image: [i0 | i1] halves cut alike
+        auto cut = [](std::vector<int> &t, std::vector<float> &f, int n, int o, int m) {
+            std::vector<int> t2((size_t)2 * m);
+            for (int k = 0; k < m; ++k) {
+                t2[k] = t[o + k];
+                t2[m + k] = t[n + o + k];
+            }
+            t.swap(t2);
+            f = std::vector<float>(f.begin() + o, f.begin() + o + m);
+        };
+        cut(tx, fx, w, sub[0], sub[2]);
+        cut(ty, fy, h, sub[1], sub[3]);
+    }
     SB_TRY(dev_alloc((void **)&gd->map, sizeof(float) * (size_t)gw * gh * gc, s));
     SB_TRY(dev_alloc((void **)&gd->tx, sizeof(int) * tx.size(), s));
     SB_TRY(dev_alloc((void **)&gd->ty, sizeof(int) * ty.size(), s));

@@ -5,6 +5,7 @@
 // fixed set of cameras.  Creation does the host geometry once (roi detection, trig tables, padded rects,
 // storage); run() enqueues warp -> pyramids -> collapse for a batch of frames without touching the host.
 #include <algorithm>
+#include <cstdlib>
 #include <cstring>
 #include <functional>
 #include <string>
@@ -32,6 +33,11 @@ struct Slot {
     // source, written by k_resize_src, in `src4` when the warp kernel reads words, else in `fin` (packed u8x3).
     std::vector<uint8_t *> fin;
     PanoOut out{};                 // device outputs
+    // timelapse (sb_compositor_create_timelapse): the pasted parts of the frames, one 16-byte aligned block per image with a
+    // non-empty part; their k_timelapse_paste jobs; the n page-locked frames of the canvas this slot's steps end in
+    uint8_t *paste = nullptr;
+    PasteJob *paste_jobs = nullptr;
+    uint8_t *frames = nullptr;
     cudaEvent_t e_h2d = nullptr, e_comp = nullptr, e_d2h = nullptr;  // submit: sources uploaded, step done, output downloaded
 #ifndef SB_EMU
     cudaGraphExec_t graph = nullptr;  // the captured step reading this slot's buffers
@@ -76,7 +82,19 @@ struct sb_compositor {
     cudaStream_t comm_stream = nullptr;
     cudaEvent_t e_part[2] = {}, e_xchg[2] = {};  // partial sums of part k written / part k received
     ShardPlan shard;
+    // timelapse mode: no blend plan; every step writes one frame of the canvas per image (cv.detail.Timelapser)
+    int timelapse = 0;                 // 0, SB_TIMELAPSE_AS_IS or SB_TIMELAPSE_CROP
+    Rect canvas{0, 0, 0, 0};           // resultRoi / resultRoiIntersection of the fed rects (pano-absolute)
+    std::vector<Rect> part;            // per image: its fed rect on the canvas (P_i, pano-absolute; w = h = 0 when empty)
+    std::vector<int> active;           // the images with a non-empty part, in warp launch order
+    std::vector<size_t> paste_off;     // per image: its block in Slot::paste
+    size_t paste_bytes = 0;
+    long long paste_max = 0;           // largest 3 * |P_i|
+    double paste_model = 0;            // model bytes of k_timelapse_paste
+    std::vector<WarpJob> tl_jobs;      // scratch: the jobs of the active images for one slot
 };
+
+static bool is_active(const sb_compositor *c, int i) { return !c->timelapse || c->part[i].w > 0; }
 
 // the sources of this rank's images and an output of slot 0's size (the panorama, or this rank's strip)
 static int slot_alloc(sb_compositor *c, Slot &sl)
@@ -86,6 +104,7 @@ static int slot_alloc(sb_compositor *c, Slot &sl)
     sl.src4.assign(c->n, nullptr);
     sl.fin.assign(c->n, nullptr);
     for (int i = c->first; i < c->first + c->count; ++i) {
+        if (!is_active(c, i)) continue;  // an image off the timelapse canvas is neither uploaded nor warped
         const long long px = (long long)c->src_w[i] * c->src_h[i];
         if (c->taps_dev[i]) {
             SB_TRY(dev_alloc((void **)&sl.src[i], (size_t)c->in_w[i] * c->in_h[i] * 3 + SB_SRC_PAD, s));
@@ -98,6 +117,20 @@ static int slot_alloc(sb_compositor *c, Slot &sl)
         SB_TRY(dev_alloc((void **)&sl.src[i], (size_t)px * 3 + SB_SRC_PAD, s));
         if (c->use_src4 && px < (1ll << 31)) SB_TRY(dev_alloc((void **)&sl.src4[i], ((size_t)px + 4) * sizeof(uint32_t), s));
     }
+    SB_CUDA(cudaEventCreateWithFlags(&sl.e_h2d, cudaEventDisableTiming));
+    SB_CUDA(cudaEventCreateWithFlags(&sl.e_comp, cudaEventDisableTiming));
+    SB_CUDA(cudaEventCreateWithFlags(&sl.e_d2h, cudaEventDisableTiming));
+    if (c->timelapse) {
+        if (c->active.empty()) return SB_OK;
+        SB_TRY(dev_alloc((void **)&sl.paste, c->paste_bytes, s));
+        std::vector<PasteJob> pj;
+        for (int i : c->active)
+            pj.push_back(PasteJob{c->rgbm_dev[i], sl.paste + c->paste_off[i], rgbm_pitch_of(c->part[i].w), c->part[i].w, c->part[i].h});
+        SB_TRY(dev_alloc((void **)&sl.paste_jobs, pj.size() * sizeof(PasteJob), s));
+        SB_CUDA(cudaMemcpyAsync(sl.paste_jobs, pj.data(), pj.size() * sizeof(PasteJob), cudaMemcpyHostToDevice, s));
+        SB_CUDA(cudaStreamSynchronize(s));  // pj goes out of scope
+        return SB_OK;
+    }
     PanoOut &o = sl.out;
     o.w = c->slots[0].out.w;
     o.h = c->slots[0].out.h;
@@ -105,9 +138,6 @@ static int slot_alloc(sb_compositor *c, Slot &sl)
     o.mask_pitch = o.w;
     SB_TRY(dev_alloc((void **)&o.rgb, (size_t)std::max(o.w, 1) * 3 * std::max(o.h, 1), s));
     SB_TRY(dev_alloc((void **)&o.mask, (size_t)std::max(o.w, 1) * std::max(o.h, 1), s));
-    SB_CUDA(cudaEventCreateWithFlags(&sl.e_h2d, cudaEventDisableTiming));
-    SB_CUDA(cudaEventCreateWithFlags(&sl.e_comp, cudaEventDisableTiming));
-    SB_CUDA(cudaEventCreateWithFlags(&sl.e_d2h, cudaEventDisableTiming));
     return SB_OK;
 }
 
@@ -118,6 +148,9 @@ static void slot_free(Slot &sl, cudaStream_t s)
     for (auto p : sl.fin) dev_free(p, s);
     dev_free(sl.out.rgb, s);
     dev_free(sl.out.mask, s);
+    dev_free(sl.paste, s);
+    dev_free(sl.paste_jobs, s);
+    if (sl.frames) (void)cudaFreeHost(sl.frames);
     for (cudaEvent_t e : {sl.e_h2d, sl.e_comp, sl.e_d2h})
         if (e) (void)cudaEventDestroy(e);
 #ifndef SB_EMU
@@ -218,12 +251,18 @@ static int check_input_sizes(const sb_rig *rig, const int *in_w, const int *in_h
 // every job of the batch has one (slot_alloc's rule); a resized image gets only the buffer that is read.
 static int plan_resize(sb_compositor *c, cudaStream_t s)
 {
-    std::vector<int> t;
-    for (int b = c->first; b < c->first + c->count; b += SB_WARP_BATCH) {
-        const int end = std::min(b + SB_WARP_BATCH, c->first + c->count);
-        bool words = warp_batch_rgbm(c->jobs.data() + b, end - b);
-        for (int i = b; i < end; ++i) words = words && c->use_src4 && (long long)c->src_w[i] * c->src_h[i] < (1ll << 31);
-        for (int i = b; i < end; ++i) {
+    std::vector<int> t, order = c->active;  // the images in launch order: a timelapse warps only those on its canvas
+    if (!c->timelapse)
+        for (int i = c->first; i < c->first + c->count; ++i) order.push_back(i);
+    std::vector<WarpJob> batch;
+    for (size_t b = 0; b < order.size(); b += SB_WARP_BATCH) {
+        const size_t end = std::min(b + SB_WARP_BATCH, order.size());
+        batch.clear();
+        for (size_t k = b; k < end; ++k) batch.push_back(c->jobs[order[k]]);
+        bool words = warp_batch_rgbm(batch.data(), (int)batch.size());
+        for (size_t k = b; k < end; ++k) words = words && c->use_src4 && (long long)c->src_w[order[k]] * c->src_h[order[k]] < (1ll << 31);
+        for (size_t k = b; k < end; ++k) {
+            const int i = order[k];
             const int w = c->src_w[i], h = c->src_h[i];
             if (c->in_w[i] == w && c->in_h[i] == h) continue;
             c->warp_src4[i] = words;
@@ -262,10 +301,57 @@ static int prepare_sources(sb_compositor *c, const Slot &sl, int i0, int i1, cud
     return c->resize_jobs.empty() ? SB_OK : launch_resize_src(c->resize_jobs.data(), (int)c->resize_jobs.size(), s);
 }
 
-// in_w / in_h: null, or the size of the frame of every image (sb_compositor_create_resized)
-static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h, int rank,
-                            int world)
+// Timelapser.initialize(corners, sizes) (timelapser.py:36-37) over what Blender.prepare would have received -- the warped
+// rects, or with a crop the crop corners and prepared sizes: the canvas is resultRoi ("as_is") or resultRoiIntersection
+// ("crop"), which builds cv::Rect(tl, br) and so returns an empty intersection as the gap between the images.  Frame i
+// shows the part P_i of fed image i that lands on the canvas; only P_i is warped (its rect in `proj` narrowed to it) and
+// pasted.  An image with an empty P_i gives an all-zero frame and no work.
+static int plan_timelapse(sb_compositor *c, int kind, const int *corners, const int *sizes, Rect *proj)
 {
+    const int n = c->n;
+    Rect &cv = c->canvas;
+    if (kind == SB_TIMELAPSE_AS_IS) {
+        cv = result_roi(corners, sizes, n);
+    } else {
+        int tlx = corners[0], tly = corners[1], brx = corners[0] + sizes[0], bry = corners[1] + sizes[1];
+        for (int i = 1; i < n; ++i) {
+            tlx = std::max(tlx, corners[2 * i]);
+            tly = std::max(tly, corners[2 * i + 1]);
+            brx = std::min(brx, corners[2 * i] + sizes[2 * i]);
+            bry = std::min(bry, corners[2 * i + 1] + sizes[2 * i + 1]);
+        }
+        cv = Rect{std::min(tlx, brx), std::min(tly, bry), std::abs(brx - tlx), std::abs(bry - tly)};
+    }
+    if (cv.w <= 0 || cv.h <= 0) {
+        // the reference's Timelapser cannot show it either: get_frame fails in convertScaleAbs
+        set_error("compositor: the timelapse canvas (%d,%d %dx%d) has a zero side", cv.x, cv.y, cv.w, cv.h);
+        return SB_ERR_INVALID;
+    }
+    c->part.assign(n, Rect{0, 0, 0, 0});
+    c->paste_off.assign(n, 0);
+    for (int i = 0; i < n; ++i) {
+        const Rect &r = c->rects[i];
+        const int x0 = std::max(r.x, cv.x), y0 = std::max(r.y, cv.y);
+        const int x1 = std::min(r.x + r.w, cv.x + cv.w), y1 = std::min(r.y + r.h, cv.y + cv.h);
+        if (x1 <= x0 || y1 <= y0) continue;
+        c->part[i] = Rect{x0, y0, x1 - x0, y1 - y0};
+        proj[i] = Rect{proj[i].x + x0 - r.x, proj[i].y + y0 - r.y, x1 - x0, y1 - y0};
+        c->active.push_back(i);
+        const long long bytes = 3ll * (x1 - x0) * (y1 - y0);
+        c->paste_off[i] = c->paste_bytes;
+        c->paste_bytes += ((size_t)bytes + 15) & ~(size_t)15;
+        c->paste_max = std::max(c->paste_max, bytes);
+        c->paste_model += 7.0 * (x1 - x0) * (y1 - y0);  // RGBM words read, u8x3 written
+    }
+    return SB_OK;
+}
+
+// in_w / in_h: null, or the size of the frame of every image (sb_compositor_create_resized); timelapse: 0 or a
+// sb_timelapse_kind (sb_compositor_create_timelapse)
+static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h, int rank,
+                            int world, int timelapse)
+{
+    c->timelapse = timelapse;
     const int n = rig->n_images;
     c->n = n;
     c->sharded = world > 1;
@@ -296,9 +382,10 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *
     c->usermask_dev.assign(n, nullptr);
     c->gain.assign(n, GainData{});
     std::vector<int> corners(2 * n), sizes(2 * n);
-    std::vector<float> host_tab;
+    std::vector<Rect> proj(n);  // the pano-absolute rect image i is warped over
+    std::vector<Projector> projs(n);
     for (int i = 0; i < n; ++i) {
-        Projector p;
+        Projector &p = projs[i];
         projector_setup(p, rig->warp_type, rig->scale, rig->K + 9 * i, rig->R + 9 * i);
         int rect[4];
         projector_roi(p, c->src_w[i], c->src_h[i], rect);
@@ -318,18 +405,25 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *
         sizes[2 * i] = rect[2];
         sizes[2 * i + 1] = rect[3];
         if (crop) {  // from here on `rect` is the part of the warped rect that is warped and fed, c->rects[i] where it is fed
-            Rect proj;
-            SB_TRY(crop_image(crop, i, c->rects[i], &proj, &c->rects[i], &sizes[2 * i]));
-            rect[0] = proj.x;
-            rect[1] = proj.y;
-            rect[2] = proj.w;
-            rect[3] = proj.h;
+            Rect slice;
+            SB_TRY(crop_image(crop, i, c->rects[i], &slice, &c->rects[i], &sizes[2 * i]));
+            rect[0] = slice.x;
+            rect[1] = slice.y;
+            rect[2] = slice.w;
+            rect[3] = slice.h;
             corners[2 * i] = c->rects[i].x;
             corners[2 * i + 1] = c->rects[i].y;
         }
+        proj[i] = Rect{rect[0], rect[1], rect[2], rect[3]};
+    }
+    if (timelapse) SB_TRY(plan_timelapse(c, timelapse, corners.data(), sizes.data(), proj.data()));
+    std::vector<float> host_tab;
+    for (int i = 0; i < n; ++i) {
+        const Projector &p = projs[i];
+        int rect[4] = {proj[i].x, proj[i].y, proj[i].w, proj[i].h};
         c->max_w = std::max(c->max_w, rect[2]);
         c->max_h = std::max(c->max_h, rect[3]);
-        if (!mine(i)) continue;  // another rank warps this image: only its geometry is needed here
+        if (!mine(i) || !is_active(c, i)) continue;  // another rank warps this image, or it is off the timelapse canvas
         SB_TRY(dev_alloc((void **)&c->rgbm_dev[i], (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
         // the row padding (never written by the warp kernel) is read by the tile kernels' 16-byte copies: weight 0
         SB_CUDA(cudaMemsetAsync(c->rgbm_dev[i], 0, (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
@@ -344,6 +438,18 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *
         c->jobs[i].dst_rgbm = c->rgbm_dev[i];
         c->jobs[i].rgbm_pitch = rgbm_pitch_of(rect[2]);
         c->warp_bytes += 3.0 * c->src_w[i] * c->src_h[i] + 4.0 * rect[2] * rect[3];
+    }
+    if (timelapse) {
+        // no blend plan: the step is warp -> paste into this slot's frames
+        SB_TRY(plan_resize(c, s));
+        SB_TRY(slot_alloc(c, c->slots[0]));
+        c->n_slots = 1;
+        for (int i : c->active) {
+            c->jobs[i].src = warp_src(c, c->slots[0], i);
+            c->jobs[i].src4 = c->slots[0].src4[i];
+        }
+        SB_CUDA(cudaStreamSynchronize(s));
+        return SB_OK;
     }
 
     // Blender.prepare (blender.py:23-38)
@@ -513,6 +619,19 @@ static int shard_local(sb_compositor *c, cudaStream_t s, const std::function<int
     return SB_OK;
 }
 
+// the jobs of the images on the timelapse canvas with `slot`'s sources (built in a scratch vector)
+static const WarpJob *timelapse_jobs_of(sb_compositor *c, int slot)
+{
+    c->tl_jobs.clear();
+    for (int i : c->active) {
+        WarpJob j = c->jobs[i];
+        j.src = warp_src(c, c->slots[slot], i);
+        j.src4 = c->slots[slot].src4[i];
+        c->tl_jobs.push_back(j);
+    }
+    return c->tl_jobs.data();
+}
+
 static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
 {
     cudaStream_t s = c->stream;
@@ -532,6 +651,13 @@ static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
         return SB_OK;
     };
     SB_TRY(mark("start"));
+    if (c->timelapse) {
+        const int na = (int)c->active.size();
+        SB_TRY(launch_warp(timelapse_jobs_of(c, slot), na, s));
+        SB_TRY(mark("warp"));
+        SB_TRY(launch_timelapse_paste(c->slots[slot].paste_jobs, na, c->paste_max, s));
+        return mark("paste");
+    }
     SB_TRY(launch_warp(slot_jobs_of(c, slot) + c->first, c->count, s));
     SB_TRY(mark("warp"));
     const PanoOut &out = c->slots[slot].out;
@@ -648,28 +774,61 @@ static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
     return SB_OK;
 }
 
-// the other slots and the copy streams of sb_compositor_submit / _wait, on the first submit
+// every slot has its buffers (and a timelapse its frames): the pipelined path may run
+static bool pipe_ready(const sb_compositor *c)
+{
+    if (c->n_slots < SB_PIPE_DEPTH) return false;
+    if (c->timelapse)
+        for (const Slot &sl : c->slots)
+            if (!sl.frames) return false;
+    return true;
+}
+
+// the other slots and the copy streams of sb_compositor_submit / _wait, on the first submit; after a failure the next
+// submit picks up where this one stopped
 static int compositor_pipe_init(sb_compositor *c)
 {
     if (!c->h2d) SB_CUDA(cudaStreamCreateWithFlags(&c->h2d, cudaStreamNonBlocking));
     if (!c->d2h) SB_CUDA(cudaStreamCreateWithFlags(&c->d2h, cudaStreamNonBlocking));
     for (; c->n_slots < SB_PIPE_DEPTH; ++c->n_slots) SB_TRY(slot_alloc(c, c->slots[c->n_slots]));
     SB_CUDA(cudaStreamSynchronize(c->stream));
+    if (c->timelapse) {
+        // the frames every timelapse step ends in: zeroed once; each step then writes only the parts P_i
+        const size_t frame = (size_t)c->canvas.w * c->canvas.h * 3, bytes = frame * c->n;
+        for (Slot &sl : c->slots) {
+            if (sl.frames) continue;
+            if (host_alloc_pinned((void **)&sl.frames, bytes) != cudaSuccess) {
+                set_error("sb_compositor_submit_timelapse: %zu bytes of page-locked memory for the frames (%d slots x %d frames of "
+                          "%dx%d x 3 bytes) could not be allocated", bytes * SB_PIPE_DEPTH, SB_PIPE_DEPTH, c->n, c->canvas.w, c->canvas.h);
+                return SB_ERR_NOMEM;
+            }
+            std::memset(sl.frames, 0, bytes);
+        }
+    }
     return SB_OK;
 }
 
-static bool valid_rig(const sb_rig *rig)
+// blend: false when the rig's blend fields are unused (a timelapse compositor)
+static bool valid_rig(const sb_rig *rig, bool blend = true)
 {
     return rig && rig->n_images > 0 && rig->n_images <= SB_MAX_IMAGES && rig->src_w && rig->src_h && rig->K && rig->R &&
-           rig->warp_type >= SB_WARP_SPHERICAL && rig->warp_type <= SB_WARP_TRANSVERSE_MERCATOR && rig->blend_kind >= SB_BLEND_NO &&
-           rig->blend_kind <= SB_BLEND_MULTIBAND;
+           rig->warp_type >= SB_WARP_SPHERICAL && rig->warp_type <= SB_WARP_TRANSVERSE_MERCATOR &&
+           (!blend || (rig->blend_kind >= SB_BLEND_NO && rig->blend_kind <= SB_BLEND_MULTIBAND));
+}
+
+// the entries that need a panorama, warped images, masks or a shard: a timelapse compositor has none of them
+static bool refuse_timelapse(const sb_compositor *c, const char *what)
+{
+    if (!c || !c->timelapse) return false;
+    set_error("%s: not available on a timelapse compositor, whose steps end in frames (sb_compositor_submit_timelapse)", what);
+    return true;
 }
 
 static sb_compositor *compositor_create(const sb_rig *rig, const sb_crop *crop, int rank, int world, const int *in_w = nullptr,
-                                        const int *in_h = nullptr)
+                                        const int *in_h = nullptr, int timelapse = 0)
 {
     sb_compositor *c = new sb_compositor;
-    if (compositor_build(c, rig, crop, in_w, in_h, rank, world) != SB_OK) {
+    if (compositor_build(c, rig, crop, in_w, in_h, rank, world, timelapse) != SB_OK) {
         compositor_free(c);
         return nullptr;
     }
@@ -720,6 +879,21 @@ sb_compositor *sb_compositor_create_resized(const sb_rig *rig, const sb_crop *cr
     return compositor_create(rig, crop, rank, world, in_w, in_h);
 }
 
+// Stitcher with timelapse="as_is" / "crop" (stitcher.py:241-252): one GPU, every step writes one frame per image
+// (plan_timelapse); crop and in_w / in_h as in sb_compositor_create_resized, both nullable
+sb_compositor *sb_compositor_create_timelapse(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h, int kind)
+{
+    if (kind != SB_TIMELAPSE_AS_IS && kind != SB_TIMELAPSE_CROP) {
+        set_error("sb_compositor_create_timelapse: unknown timelapse kind %d", kind);
+        return nullptr;
+    }
+    if (!valid_rig(rig, false) || !in_w != !in_h || (crop && (!crop->rect || !crop->corner || !crop->size))) {
+        set_error("sb_compositor_create_timelapse: invalid argument");
+        return nullptr;
+    }
+    return compositor_create(rig, crop, 0, 1, in_w, in_h, kind);
+}
+
 int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_local, int strip[2])
 {
     if (!c) {
@@ -730,7 +904,7 @@ int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_lo
     if (n_local) *n_local = c->count;
     if (strip) {
         strip[0] = 0;
-        strip[1] = c->plan.roi.w;
+        strip[1] = c->timelapse ? c->canvas.w : c->plan.roi.w;
         if (c->sharded) c->shard.strip(c->plan, &strip[0], &strip[1]);  // columns, or rows when sb_compositor_shard_axis() == 1
     }
     return SB_OK;
@@ -740,6 +914,7 @@ int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_lo
 // move the slabs itself (tests do, with plain copies; sb_compositor_run uses NCCL).
 int sb_compositor_shard_phase(sb_compositor *c, int phase)
 {
+    if (refuse_timelapse(c, "sb_compositor_shard_phase")) return SB_ERR_STATE;
     if (!c || !c->sharded || phase < 0 || phase > 1) {
         set_error("sb_compositor_shard_phase: invalid argument");
         return SB_ERR_INVALID;
@@ -762,6 +937,7 @@ int sb_compositor_shard_axis(const sb_compositor *c) { return c && c->sharded ? 
 
 int sb_compositor_shard_slab(sb_compositor *c, int peer, int outgoing, void **dev_ptr, size_t *bytes)
 {
+    if (refuse_timelapse(c, "sb_compositor_shard_slab")) return SB_ERR_STATE;
     if (!c || !c->sharded || peer < 0 || peer >= c->shard.world || peer == c->shard.rank || !dev_ptr || !bytes) {
         set_error("sb_compositor_shard_slab: invalid argument");
         return SB_ERR_INVALID;
@@ -788,12 +964,13 @@ int sb_compositor_geometry(const sb_compositor *c, int *rects, int pano_roi[4], 
             rects[4 * i + 3] = c->rects[i].h;
         }
     if (pano_roi) {
-        pano_roi[0] = c->plan.roi.x;
-        pano_roi[1] = c->plan.roi.y;
-        pano_roi[2] = c->plan.roi.w;
-        pano_roi[3] = c->plan.roi.h;
+        const Rect &r = c->timelapse ? c->canvas : c->plan.roi;  // a timelapse: its canvas
+        pano_roi[0] = r.x;
+        pano_roi[1] = r.y;
+        pano_roi[2] = r.w;
+        pano_roi[3] = r.h;
     }
-    if (num_bands) *num_bands = c->plan.kind == SB_BLEND_MULTIBAND ? c->plan.nb : -1;
+    if (num_bands) *num_bands = !c->timelapse && c->plan.kind == SB_BLEND_MULTIBAND ? c->plan.nb : -1;
     return SB_OK;
 }
 
@@ -805,7 +982,10 @@ int sb_compositor_model_bytes(const sb_compositor *c, double *total_bytes, doubl
     }
     std::vector<double> v;
     v.push_back(c->warp_bytes);
-    for (const auto &kv : c->plan.launch_bytes()) v.push_back(kv.second);
+    if (c->timelapse)
+        v.push_back(c->paste_model);
+    else
+        for (const auto &kv : c->plan.launch_bytes()) v.push_back(kv.second);
     double tot = 0;
     for (double b : v) tot += b;
     if (total_bytes) *total_bytes = tot;
@@ -816,6 +996,7 @@ int sb_compositor_model_bytes(const sb_compositor *c, double *total_bytes, doubl
 
 int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pitch, int pinned)
 {
+    if (refuse_timelapse(c, "sb_compositor_upload")) return SB_ERR_STATE;
     if (!c || i < 0 || i >= c->n || !src || pitch < (size_t)c->in_w[i] * 3) {
         set_error("sb_compositor_upload: invalid argument");
         return SB_ERR_INVALID;
@@ -834,6 +1015,7 @@ int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pit
 
 int sb_compositor_set_mask(sb_compositor *c, int i, const uint8_t *mask, size_t pitch)
 {
+    if (refuse_timelapse(c, "sb_compositor_set_mask")) return SB_ERR_STATE;  // the Timelapser ignores masks
     if (!c || i < 0 || i >= c->n || !mask || pitch < (size_t)c->rects[i].w || !c->rgbm_dev[i]) {
         set_error("sb_compositor_set_mask: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
@@ -850,6 +1032,7 @@ int sb_compositor_set_mask(sb_compositor *c, int i, const uint8_t *mask, size_t 
 
 int sb_compositor_set_seam_mask(sb_compositor *c, int i, const uint8_t *seam, size_t seam_pitch, int sw, int sh)
 {
+    if (refuse_timelapse(c, "sb_compositor_set_seam_mask")) return SB_ERR_STATE;
     if (!c || i < 0 || i >= c->n || !seam || sw <= 0 || sh <= 0 || seam_pitch < (size_t)sw || !c->rgbm_dev[i]) {
         set_error("sb_compositor_set_seam_mask: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
@@ -866,16 +1049,24 @@ int sb_compositor_set_seam_mask(sb_compositor *c, int i, const uint8_t *seam, si
 
 int sb_compositor_set_gain(sb_compositor *c, int i, const float *gain_map, int gw, int gh, int gc, const double *gain_scalar)
 {
-    if (!c || i < 0 || i >= c->n || !c->rgbm_dev[i] || (gain_map && gain_scalar) ||
+    if (!c || i < 0 || i >= c->n || (!c->rgbm_dev[i] && !c->timelapse) || (gain_map && gain_scalar) ||
         (gain_map && (gw <= 0 || gh <= 0 || (gc != 1 && gc != 3)))) {
         set_error("sb_compositor_set_gain: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
     }
+    if (!is_active(c, i)) return SB_OK;  // off the timelapse canvas: nothing of it is shown
     // ExposureErrorCompensator.apply(i, corner, warped image, mask) (exposure_error_compensator.py:43-45,
     // stitcher.py:219-221) fused into the warp's epilogue: the warped image never exists uncompensated
     SB_CUDA(cudaStreamSynchronize(c->stream));  // the previous run may still read the old gain buffers
     drop_graphs(c);  // before the upload, which frees the buffers they read
-    return gain_upload(&c->jobs[i], &c->gain[i], c->rects[i].w, c->rects[i].h, gain_map, gw, gh, gc, gain_scalar, c->stream);
+    const Rect &r = c->rects[i];
+    if (c->timelapse) {
+        // only P_i is warped, but the gain map is resized to the whole fed image: the taps at P_i's place in it
+        const Rect &p = c->part[i];
+        const int sub[4] = {p.x - r.x, p.y - r.y, p.w, p.h};
+        return gain_upload(&c->jobs[i], &c->gain[i], r.w, r.h, gain_map, gw, gh, gc, gain_scalar, c->stream, sub);
+    }
+    return gain_upload(&c->jobs[i], &c->gain[i], r.w, r.h, gain_map, gw, gh, gc, gain_scalar, c->stream);
 }
 
 int sb_compositor_run(sb_compositor *c)
@@ -884,6 +1075,7 @@ int sb_compositor_run(sb_compositor *c)
         set_error("sb_compositor_run: null handle");
         return SB_ERR_INVALID;
     }
+    if (refuse_timelapse(c, "sb_compositor_run")) return SB_ERR_STATE;
     return compositor_enqueue(c, false);
 }
 
@@ -896,6 +1088,7 @@ int sb_compositor_sync(sb_compositor *c)
 
 int sb_compositor_download(sb_compositor *c, uint8_t *dst, size_t dst_pitch, uint8_t *dst_mask, size_t mask_pitch)
 {
+    if (refuse_timelapse(c, "sb_compositor_download")) return SB_ERR_STATE;
     if (!c || (dst && dst_pitch < (size_t)c->slots[0].out.w * 3) || (dst_mask && mask_pitch < (size_t)c->slots[0].out.w)) {
         set_error("sb_compositor_download: invalid argument");
         return SB_ERR_INVALID;
@@ -910,6 +1103,7 @@ int sb_compositor_download(sb_compositor *c, uint8_t *dst, size_t dst_pitch, uin
 int sb_compositor_submit(sb_compositor *c, const uint8_t *const *srcs, const size_t *pitches, uint8_t *dst, size_t dst_pitch,
                          uint8_t *dst_mask, size_t mask_pitch, unsigned long long *ticket)
 {
+    if (refuse_timelapse(c, "sb_compositor_submit")) return SB_ERR_STATE;
     if (!c || !srcs || !pitches || (dst && dst_pitch < (size_t)c->slots[0].out.w * 3) || (dst_mask && mask_pitch < (size_t)c->slots[0].out.w)) {
         set_error("sb_compositor_submit: invalid argument");
         return SB_ERR_INVALID;
@@ -962,8 +1156,72 @@ int sb_compositor_wait(sb_compositor *c, unsigned long long ticket)
     return SB_OK;
 }
 
+// Pipelined timelapse step: H2D of the images on the canvas, warp + paste, then one 2D copy per image from its pasted part
+// into its frame of this slot at P_i (the rest of every frame stays zero).  The ticket works with sb_compositor_wait.
+int sb_compositor_submit_timelapse(sb_compositor *c, const uint8_t *const *srcs, const size_t *pitches, unsigned long long *ticket)
+{
+    if (!c || !srcs || !pitches) {
+        set_error("sb_compositor_submit_timelapse: invalid argument");
+        return SB_ERR_INVALID;
+    }
+    if (!c->timelapse) {
+        set_error("sb_compositor_submit_timelapse: not a timelapse compositor (sb_compositor_create_timelapse)");
+        return SB_ERR_STATE;
+    }
+    for (int i = 0; i < c->n; ++i)
+        if (!srcs[i] || pitches[i] < (size_t)c->in_w[i] * 3) {
+            set_error("sb_compositor_submit_timelapse: invalid source %d", i);
+            return SB_ERR_INVALID;
+        }
+    if (!pipe_ready(c)) SB_TRY(compositor_pipe_init(c));
+    const unsigned long long t = c->submitted;
+    const int slot = (int)(t % SB_PIPE_DEPTH);
+    Slot &sl = c->slots[slot];
+    // as in sb_compositor_submit: the sources are free once the previous compute that read them has finished
+    if (t < SB_PIPE_DEPTH) SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
+    SB_CUDA(cudaStreamWaitEvent(c->h2d, sl.e_comp, 0));
+    for (int i : c->active)
+        SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->in_w[i] * 3, srcs[i], pitches[i], (size_t)c->in_w[i] * 3, c->in_h[i],
+                          cudaMemcpyHostToDevice, c->h2d));
+    SB_TRY(prepare_sources(c, sl, 0, c->n, c->h2d));
+    SB_CUDA(cudaEventRecord(sl.e_h2d, c->h2d));
+    SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_h2d, 0));
+    // the paste buffer of this slot is free once its previous download has finished
+    if (t >= SB_PIPE_DEPTH) SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_d2h, 0));
+    SB_TRY(compositor_enqueue(c, false, slot));
+    SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
+    SB_CUDA(cudaStreamWaitEvent(c->d2h, sl.e_comp, 0));
+    const Rect &cv = c->canvas;
+    const size_t fpitch = (size_t)cv.w * 3, fbytes = fpitch * cv.h;
+    for (int i : c->active) {
+        const Rect &p = c->part[i];
+        uint8_t *dst = sl.frames + fbytes * i + (size_t)(p.y - cv.y) * fpitch + (size_t)(p.x - cv.x) * 3;
+        SB_CUDA(sb_copy2d(dst, fpitch, sl.paste + c->paste_off[i], (size_t)p.w * 3, (size_t)p.w * 3, p.h, cudaMemcpyDeviceToHost, c->d2h));
+    }
+    SB_CUDA(cudaEventRecord(sl.e_d2h, c->d2h));
+    c->submitted = t + 1;
+    if (ticket) *ticket = t;
+    return SB_OK;
+}
+
+int sb_compositor_timelapse_frame(const sb_compositor *c, unsigned long long ticket, int i, const uint8_t **frame, size_t *pitch)
+{
+    if (!c || i < 0 || i >= c->n || !frame || !pitch) {
+        set_error("sb_compositor_timelapse_frame: invalid argument");
+        return SB_ERR_INVALID;
+    }
+    if (!c->timelapse || !pipe_ready(c) || ticket >= c->submitted || ticket + SB_PIPE_DEPTH < c->submitted) {
+        set_error("sb_compositor_timelapse_frame: ticket %llu is not in flight on a timelapse compositor", ticket);
+        return SB_ERR_STATE;
+    }
+    *pitch = (size_t)c->canvas.w * 3;
+    *frame = c->slots[ticket % SB_PIPE_DEPTH].frames + *pitch * c->canvas.h * i;
+    return SB_OK;
+}
+
 int sb_compositor_download_warped(sb_compositor *c, int i, uint8_t *dst, size_t dst_pitch, uint8_t *dst_mask, size_t mask_pitch)
 {
+    if (refuse_timelapse(c, "sb_compositor_download_warped")) return SB_ERR_STATE;
     if (!c || i < 0 || i >= c->n || !c->rgbm_dev[i]) {
         set_error("sb_compositor_download_warped: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
@@ -996,6 +1254,8 @@ int sb_compositor_time_multi(sb_compositor *const *cs, int n, int iters, float *
         set_error("sb_compositor_time_multi: invalid argument");
         return SB_ERR_INVALID;
     }
+    for (int k = 0; k < n; ++k)
+        if (refuse_timelapse(cs[k], "sb_compositor_time_multi")) return SB_ERR_STATE;
     for (int k = 0; k < n; ++k)
         if (!cs[k] || cs[k]->sharded) {
             set_error("sb_compositor_time_multi: null or sharded compositor");

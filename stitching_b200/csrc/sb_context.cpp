@@ -166,8 +166,7 @@ void *sb_host_alloc(size_t bytes)
 {
     if (sb::ensure_device() != SB_OK) return nullptr;
     void *p = nullptr;
-    if (cudaMallocHost(&p, bytes) != cudaSuccess) {
-        (void)cudaGetLastError();
+    if (sb::host_alloc_pinned(&p, bytes) != cudaSuccess) {
         sb::set_error("cudaMallocHost(%zu) failed", bytes);
         return nullptr;
     }
@@ -181,6 +180,21 @@ void sb_host_free(void *p)
 }  // extern "C"
 
 namespace sb {
+// SB_PINNED_MAX_BYTES=<bytes>: a request for more page-locked memory than that fails as if the host had none left (a cap
+// for shared hosts; read on every call)
+cudaError_t host_alloc_pinned(void **p, size_t bytes)
+{
+    *p = nullptr;
+    const char *e = getenv("SB_PINNED_MAX_BYTES");
+    if (e && *e && bytes > (size_t)strtoull(e, nullptr, 10)) return cudaErrorMemoryAllocation;
+    const cudaError_t r = cudaMallocHost(p, bytes);
+    if (r != cudaSuccess) {
+        (void)cudaGetLastError();
+        *p = nullptr;
+    }
+    return r;
+}
+
 bool pdl_enabled()
 {
     static const bool on = [] {

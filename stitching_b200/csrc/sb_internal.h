@@ -39,6 +39,8 @@ void count_launch(unsigned n = 1);
 void adjust_launch_count(long long delta);  // graph capture records launches that do not execute; replays execute them
 cudaStream_t default_stream();
 
+// page-locked host memory (cudaMallocHost), capped by SB_PINNED_MAX_BYTES when it is set (sb_context.cpp)
+cudaError_t host_alloc_pinned(void **p, size_t bytes);
 // stream-ordered device allocation (cudaMallocAsync pool with a high release threshold)
 int dev_alloc(void **p, size_t bytes, cudaStream_t s);
 void dev_free(void *p, cudaStream_t s);
@@ -292,6 +294,15 @@ static inline cudaError_t sb_copy2d(void *dst, size_t dpitch, const void *src, s
 // Timelapser frame: src8 (uint8 x3, pitch in bytes) or src16 (int16 x3, pitch in ELEMENTS) pasted at (dx, dy) of a cw x ch canvas
 int launch_timelapse_frame(const uint8_t *src8, const int16_t *src16, long long spitch, int sw, int sh, int dx, int dy, uint8_t *dst,
                            long long dpitch, int cw, int ch, cudaStream_t s);
+// one image of k_timelapse_paste: the warped part of a timelapse frame (rgbm, w x h words) as dense u8x3 rows of w * 3
+// bytes at dst (16-byte aligned)
+struct PasteJob {
+    const uint32_t *rgbm;
+    uint8_t *dst;
+    long long rgbm_pitch;  // elements
+    int w, h;
+};
+int launch_timelapse_paste(const PasteJob *jobs_dev, int n_jobs, long long max_bytes, cudaStream_t s);  // one launch for all
 int launch_gain_apply(uint8_t *img, long long pitch, int w, int h, const WarpJob &gain_fields, cudaStream_t s);
 // device copies of one image's gain (map + taps for a w x h target, or the scalar tables) and the WarpJob fields for them
 struct GainData {
@@ -299,8 +310,10 @@ struct GainData {
     int *tx = nullptr, *ty = nullptr;
     uint8_t *lut = nullptr;
 };
+// sub (nullable): only the rect sub = (x, y, w', h') of the w x h image is warped; the map is still resized to w x h and the
+// job indexes the taps of that rect's columns and rows
 int gain_upload(WarpJob *job, GainData *gd, int w, int h, const float *gain_map, int gw, int gh, int gc, const double *gain_scalar,
-                cudaStream_t s);  // synchronises s
+                cudaStream_t s, const int *sub = nullptr);  // synchronises s
 void gain_free(GainData *gd, cudaStream_t s);
 // Images.resize_img_by_scaler: cv.resize(uint8, INTER_LINEAR_EXACT) (sb_seam.cu, sb_geometry.cpp)
 void resize_exact_taps(int n_src, int n_dst, int *t);  // t: 3 * n_dst ints

@@ -122,6 +122,53 @@ int launch_timelapse_frame(const uint8_t *src8, const int16_t *src16, long long 
     return launch_check("k_timelapse_frame");
 }
 
+// The timelapse compositor's step after the warp: image blockIdx.z's warped words (r | g << 8 | b << 16 | mask << 24) become
+// dense u8x3 rows of w * 3 bytes -- the part of its frame that lands on the canvas, ready for one 2D copy to the host.  The
+// image's bytes are one stream: each thread writes 16 consecutive bytes of it with one aligned 16-byte store (the last,
+// partial group byte by byte), reading the 6 or 7 words they come from.  Nothing else of the frame is written: the
+// zeros around it never change on the host.
+__global__ void __launch_bounds__(256) k_timelapse_paste(const PasteJob *__restrict__ jobs)
+{
+    grid_dependency_sync();
+    const PasteJob j = jobs[blockIdx.z];
+    const long long bytes = 3ll * j.w * j.h;
+    for (long long b0 = 16ll * (blockIdx.x * (long long)blockDim.x + threadIdx.x); b0 < bytes; b0 += 16ll * gridDim.x * blockDim.x) {
+        const long long p = b0 / 3;
+        int c = (int)(b0 - 3 * p), y = (int)(p / j.w), x = (int)(p - (long long)y * j.w);
+        const uint32_t *row = j.rgbm + (long long)y * j.rgbm_pitch;
+        const int nb = bytes - b0 < 16 ? (int)(bytes - b0) : 16;
+        unsigned out[4] = {0u, 0u, 0u, 0u}, word = row[x];
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+            if (k < nb) out[k >> 2] |= ((word >> (8 * c)) & 255u) << (8 * (k & 3));
+            if (++c == 3) {
+                c = 0;
+                if (++x == j.w) {
+                    x = 0;
+                    row += j.rgbm_pitch;
+                }
+                if (k + 1 < nb) word = row[x];
+            }
+        }
+        if (nb == 16) {
+            *reinterpret_cast<uint4 *>(j.dst + b0) = make_uint4(out[0], out[1], out[2], out[3]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 16; ++k)  // unrolled: out[] stays in registers
+                if (k < nb) j.dst[b0 + k] = (uint8_t)(out[k >> 2] >> (8 * (k & 3)));
+        }
+    }
+}
+
+// max_bytes: the largest 3 * w * h of the jobs
+int launch_timelapse_paste(const PasteJob *jobs_dev, int n_jobs, long long max_bytes, cudaStream_t s)
+{
+    if (n_jobs <= 0 || max_bytes <= 0) return SB_OK;
+    const int bx = (int)std::min<long long>((max_bytes + 16ll * 256 - 1) / (16ll * 256), 1 << 20);
+    launch_pdl(k_timelapse_paste, dim3(bx, 1, n_jobs), dim3(256), 0, s, jobs_dev);
+    return launch_check("k_timelapse_paste");
+}
+
 // overwrite a buffer larger than L2 so that the next kernel starts from a cold cache
 int launch_flush_l2(void *buf, size_t bytes, cudaStream_t s)
 {
