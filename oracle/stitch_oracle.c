@@ -983,6 +983,9 @@ SO_API void so_resize_linear_f32(const float *src, int sw, int sh, int cn, int d
 static uint8_t sat_round_u8(double v) /* saturate_cast<uchar>(cvRound(v)) */
 {
     const double r = nearbyint(v);
+    /* cvRound is cvtss2si / cvtsd2si: INT_MIN when the rounded value is not an int (NaN included), which saturates to 0
+     * (golden_gain_range.npz, written by the reference's compensators) */
+    if (!(r >= -2147483648.0 && r <= 2147483647.0)) return 0;
     return (uint8_t)(r < 0 ? 0 : (r > 255 ? 255 : r));
 }
 

@@ -511,13 +511,15 @@ void resize_exact_taps(int n_src, int n_dst, int *t)
 }
 
 // GainCompensator / ChannelsCompensator::apply multiply by a double scalar: saturate_cast<uchar>(cvRound(v * gain)),
-// tabulated for the 256 byte values of each channel
+// tabulated for the 256 byte values of each channel.  cvRound is cvtsd2si: a product whose rounded value is not an int
+// (NaN included) becomes INT_MIN, which saturates to 0.
 void gain_scalar_lut(const double gain[3], uint8_t lut[768])
 {
     for (int c = 0; c < 3; ++c)
         for (int v = 0; v < 256; ++v) {
             const double r = std::nearbyint((double)v * gain[c]);
-            lut[c * 256 + v] = (uint8_t)(r < 0 ? 0 : (r > 255 ? 255 : r));
+            const bool is_int = r >= -2147483648.0 && r <= 2147483647.0;
+            lut[c * 256 + v] = (uint8_t)(!is_int || r < 0 ? 0 : (r > 255 ? 255 : r));
         }
 }
 

@@ -77,7 +77,9 @@ __device__ __forceinline__ void apply_gain(const WarpJob &j, int u, int v, unsig
             const float h0 = fmaf(fadd(b0, -a0), fx, a0), h1 = fmaf(fadd(b1, -a1), fx, a1);
             gain = fmaf(fadd(h1, -h0), fy, h0);
         }
-        const int q = __float2int_rn(fmul((float)c[k], gain));  // |value * gain| is far below 2^31
+        // cvRound(float) is cvtss2si: INT_MIN (so 0 after saturation) when the product leaves the int range or is NaN,
+        // which set_gain's maps can make it; the device's saturating cvt would give 255
+        const int q = cvt_rn_x86(fmul((float)c[k], gain));
         c[k] = (unsigned)sat_u8(q);
     }
     r = c[0];

@@ -70,9 +70,18 @@ static inline cudaError_t cudaStreamDestroy(cudaStream_t s) { std::free(s); retu
 static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
 static inline cudaError_t cudaDeviceGetDefaultMemPool(cudaMemPool_t *p, int) { *p = 0; return cudaSuccess; }
 static inline cudaError_t cudaMemPoolSetAttribute(cudaMemPool_t, cudaMemPoolAttr, void *) { return cudaSuccess; }
-static inline cudaError_t cudaMallocAsync(void **p, size_t n, cudaStream_t) { *p = std::malloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+// SB_EMU_FILL=<byte> (e.g. 0xff): every new device and page-locked allocation starts filled with that byte instead of
+// whatever malloc returns (large blocks are fresh zero pages, which hide reads of memory no step wrote).  Unset: no fill.
+static inline void *emu_alloc(size_t n)
+{
+    void *p = std::malloc(n);
+    const char *fill = std::getenv("SB_EMU_FILL");
+    if (p && fill && *fill) std::memset(p, (int)(std::strtol(fill, nullptr, 0) & 0xff), n);
+    return p;
+}
+static inline cudaError_t cudaMallocAsync(void **p, size_t n, cudaStream_t) { *p = emu_alloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 static inline cudaError_t cudaFreeAsync(void *p, cudaStream_t) { std::free(p); return cudaSuccess; }
-static inline cudaError_t cudaMallocHost(void **p, size_t n) { *p = std::malloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
+static inline cudaError_t cudaMallocHost(void **p, size_t n) { *p = emu_alloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 static inline cudaError_t cudaFreeHost(void *p) { std::free(p); return cudaSuccess; }
 static inline cudaError_t cudaMemsetAsync(void *d, int v, size_t n, cudaStream_t) { std::memset(d, v, n); return cudaSuccess; }
 static inline cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, cudaMemcpyKind, cudaStream_t) { std::memcpy(d, s, n); return cudaSuccess; }
@@ -121,8 +130,11 @@ static inline unsigned __byte_perm(unsigned a, unsigned b, unsigned sel)
     return r;
 }
 static inline unsigned __dp2a_lo(unsigned a, unsigned b, unsigned c) { return c + (a & 0xffffu) * (b & 0xffu) + (a >> 16) * ((b >> 8) & 0xffu); }
-static inline int __float2int_rn(float v) { return (int)nearbyintf(v); }
-static inline int __float2int_rz(float v) { return (int)v; }
+// cvt.rni / cvt.rzi .s32.f32 saturate: NaN gives 0, values beyond the int range its nearest end (a plain (int) cast
+// would be undefined there, and x86 gives INT_MIN)
+static inline int emu_sat_s32(float r) { return r != r ? 0 : r >= 2147483648.f ? INT32_MAX : r < -2147483648.f ? INT32_MIN : (int)r; }
+static inline int __float2int_rn(float v) { return emu_sat_s32(nearbyintf(v)); }
+static inline int __float2int_rz(float v) { return emu_sat_s32(truncf(v)); }
 static inline int min(int a, int b) { return a < b ? a : b; }
 static inline int max(int a, int b) { return a > b ? a : b; }
 

@@ -384,3 +384,43 @@ def fused_gain_case(oracle, Warper, Blender, Compositor, rigs, scale_down, kinds
     pano0, _ = c.composite(imgs)
     c.close()
     return (pano, mask), (ref_pano, ref_mask), pano0
+
+
+def run_gain_range_golden(oracle, apply_fn, Warper, Blender, Compositor, rigs, scale_down):
+    """Gains whose products value * gain leave the int range (tests/golden/golden_gain_range.npz, written by the
+    reference's compensators): cvRound rounds such a product -- and NaN -- to INT_MIN, which saturates to 0, not 255.
+    The oracle and apply_fn(img, gain) against the reference on 1- and 3-channel maps and scalars; a channel vector of
+    such gains against the oracle; and the same gains set on a compositor (applied in the warp kernel) against warp ->
+    oracle.gain_apply -> Blender."""
+    z = load("golden_gain_range.npz")
+    img = z["img"]
+    cases = [(n, z[n], z[n + "_out"]) for n in ("map1", "map3")]
+    cases += [(f"scalar {g}", np.array([[g]], np.float64), z[f"scalar{k}_out"]) for k, g in enumerate(z["scalars"])]
+    for name, gain, want in cases:
+        assert_exact(oracle.gain_apply(img, gain), want, f"oracle, gain {name}")
+        assert_exact(np.asarray(apply_fn(img.copy(), gain)), want, f"apply, gain {name}")
+    vec = np.array([[1.0e7], [np.nan], [8.5e6], [0.0]], np.float64)
+    assert_exact(np.asarray(apply_fn(img.copy(), vec)), oracle.gain_apply(img, vec), "apply, channel gains out of range")
+    gains = [z["map1"], z["map3"], np.array([[1.0e7]], np.float64), vec, None]
+    cfg = rigs.config("cfg2", scale_down)
+    cams = cfg["cameras"][: len(gains)]
+    sizes_in = [(cfg["w"], cfg["h"])] * len(cams)
+    imgs = [rigs.synth_image(cfg["h"], cfg["w"], 70 + i) for i in range(len(cams))]
+    w = Warper(cfg["warper"])
+    w.set_scale(cams)
+    corners, sizes = w.warp_rois(sizes_in, cams)
+    b = Blender(cfg["blender"], cfg["strength"])
+    b.prepare(corners, sizes)
+    for i in range(len(cams)):
+        wi, wm = w.warp_image_and_mask(imgs[i], cams[i])
+        b.feed(oracle.gain_apply(wi, gains[i]) if gains[i] is not None else wi, wm, corners[i])
+    ref = b.blend()
+    c = Compositor(cams, sizes_in, cfg["warper"], cfg["blender"], cfg["strength"])
+    try:
+        for i, g in enumerate(gains):
+            c.set_gain(i, g)
+        got = c.composite(imgs)
+    finally:
+        c.close()
+    assert_exact(got[0], ref[0], "pano with gains out of the int range")
+    assert_exact(got[1], ref[1], "mask with gains out of the int range")

@@ -505,6 +505,14 @@ def test_exposure_gain_drop_in_and_fused(use_emu, oracle):
     assert not np.array_equal(got[0], pano0), "removing a gain must change the panorama back"
 
 
+
+def test_gains_out_of_the_int_range(use_emu, oracle):
+    """Gain maps and scalars whose products leave the int range (or are NaN): 0 where cvRound gives INT_MIN, as the
+    reference's compensators do, in ExposureErrorCompensator.apply and in the compositor's warp kernel."""
+    from stitching_b200 import exposure_error_compensator as ec
+
+    replay.run_gain_range_golden(oracle, ec.apply_gain, Warper, Blender, Compositor, rigs, 25)
+
 def _twin_chain(oracle):
     """warp -> crop (slicing, cropper.py:150-151) -> ExposureErrorCompensator.apply -> Blender.feed / blend with the warped
     images' device twins, against the same chain on plain host copies of the same arrays."""

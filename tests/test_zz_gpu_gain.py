@@ -23,6 +23,11 @@ def test_gain_apply_goldens_and_fuzz(cuda_lib, oracle):
         replay.assert_exact(ec.apply_gain(img.copy(), gain), oracle.gain_apply(img, gain), f"gain fuzz {t}")
 
 
+
+def test_gains_out_of_the_int_range(cuda_lib, oracle):
+    """Products beyond the int range and NaN round to INT_MIN (so 0) as on x86, not to the device's saturated 255."""
+    replay.run_gain_range_golden(oracle, ec.apply_gain, Warper, Blender, Compositor, rigs, 4)
+
 def test_fused_final_resolution_chain(cuda_lib, oracle):
     """Gains and seam masks together in the fast warp kernel's extras path."""
     got, ref = replay.fused_chain_case(oracle, Warper, Blender, Compositor, rigs, 4)
