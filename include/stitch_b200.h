@@ -180,11 +180,7 @@ typedef struct {
     const int *src_h;     /* [n] */
     const float *K;       /* [n][9] */
     const float *R;       /* [n][9] */
-    int mask_mode;        /* 0: blend mask = warped validity mask (seam finder "no"); 1: masks supplied via sb_compositor_set_mask */
 } sb_rig;
-
-SB_API sb_compositor *sb_compositor_create(const sb_rig *rig);
-SB_API void sb_compositor_destroy(sb_compositor *c);
 
 /* The crop of Stitcher's default Cropper (cropper.py), in FINAL pixels: image i feeds the slice `rect` of its warped
  * image at `corner`, and Blender.prepare sees `size`.  The pano roi and num_bands follow the prepared sizes. */
@@ -194,29 +190,40 @@ typedef struct {
     const int *corner;  /* [n][2] Blender.feed corner of image i (Cropper.crop_rois) */
     const int *size;    /* [n][2] size of image i as Blender.prepare receives it (Cropper.crop_rois) */
 } sb_crop;
-/* sb_compositor_create (world == 1) or sb_compositor_create_sharded with a crop; crop == NULL crops nothing.  A negative
- * offset or size, an empty slice or a slice larger than its prepared size fails (SB_ERR_INVALID, named in sb_last_error):
- * the reference's blenders cannot feed an empty image either. */
-SB_API sb_compositor *sb_compositor_create_cropped(const sb_rig *rig, const sb_crop *crop, int rank, int world);
-/* sb_compositor_create_cropped (crop may be NULL) taking camera-resolution frames, as Stitcher does when final_megapix is
- * set: sb_compositor_upload / _submit take image i as in_w[i] x in_h[i], and the library resizes it on the device to its
- * FINAL size rig->src_w[i] x rig->src_h[i] (what is warped) exactly as Images.resize_img_by_scaler does
- * (cv.resize INTER_LINEAR_EXACT).  An image whose two sizes are equal is taken as it is.  An input size that is not
- * positive, smaller than the FINAL size on either axis (the reference never scales up) or with a side of 32767 px or
- * more fails (SB_ERR_INVALID, the image named in sb_last_error). */
-SB_API sb_compositor *sb_compositor_create_resized(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h,
-                                                   int rank, int world);
-/* Stitcher with timelapse="as_is" / "crop" (stitcher.py:241-252, timelapser.py): instead of a panorama, every step writes
- * one frame per image -- cv.detail.Timelapser's canvas, zero except for the fed image i (warped, cropped and compensated)
- * pasted at its corner.  The canvas is resultRoi (AS_IS) or resultRoiIntersection (CROP, an empty intersection giving the
- * gap between the images) of what Blender.prepare would have received.  crop, in_w / in_h (both nullable) as in
- * sb_compositor_create_resized; one GPU; rig->blend_* are unused.  A canvas with a zero side, which the reference's
- * get_frame cannot show, fails (SB_ERR_INVALID).  sb_compositor_geometry returns the fed rects, the canvas as pano_roi and
- * num_bands = -1; set_gain, wait, sync, time, stage_times and model_bytes work; upload, run, download, download_warped,
- * submit, set_mask, set_seam_mask, time_multi and the shard hooks fail with SB_ERR_STATE. */
 typedef enum { SB_TIMELAPSE_AS_IS = 1, SB_TIMELAPSE_CROP = 2 } sb_timelapse_kind;
-SB_API sb_compositor *sb_compositor_create_timelapse(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h,
-                                                     int kind);
+
+/* What a compositor does besides warping and blending the rig's FINAL-size images into a panorama on one GPU:
+ *   crop       every image cropped as Stitcher.crop_final_resolution does; NULL crops nothing.  A negative offset or size,
+ *              an empty slice or a slice larger than its prepared size fails (SB_ERR_INVALID, named in sb_last_error):
+ *              the reference's blenders cannot feed an empty image either.
+ *   in_w, in_h camera-resolution frames, as Stitcher takes them when final_megapix is set: sb_compositor_upload / _submit
+ *              take image i as in_w[i] x in_h[i], and the library resizes it on the device to its FINAL size
+ *              rig->src_w[i] x rig->src_h[i] (what is warped) exactly as Images.resize_img_by_scaler does
+ *              (cv.resize INTER_LINEAR_EXACT).  An image whose two sizes are equal is taken as it is.  An input size that
+ *              is not positive, smaller than the FINAL size on either axis (the reference never scales up) or with a side
+ *              of 32767 px or more fails (SB_ERR_INVALID, the image named in sb_last_error).  Both or neither.
+ *   rank, world one panorama over `world` GPUs, see the multi-GPU section below; 0, 1 for one GPU.
+ *   timelapse  Stitcher with timelapse="as_is" / "crop" (stitcher.py:241-252, timelapser.py): instead of a panorama,
+ *              every step writes one frame per image -- cv.detail.Timelapser's canvas, zero except for the fed image i
+ *              (warped, cropped and compensated) pasted at its corner.  The canvas is resultRoi (AS_IS) or
+ *              resultRoiIntersection (CROP, an empty intersection giving the gap between the images) of what
+ *              Blender.prepare would have received.  One GPU; rig->blend_* are unused.  A canvas with a zero side, which
+ *              the reference's get_frame cannot show, fails (SB_ERR_INVALID).  sb_compositor_geometry returns the fed
+ *              rects, the canvas as pano_roi and num_bands = -1; set_gain, wait, sync, time, stage_times and model_bytes
+ *              work; upload, run, download, download_warped, submit, set_mask, set_seam_mask, time_multi and the shard
+ *              hooks fail with SB_ERR_STATE. */
+typedef struct {
+    const sb_crop *crop;    /* nullable */
+    const int *in_w, *in_h; /* both or neither */
+    int rank, world;        /* world >= 1 */
+    int timelapse;          /* 0, SB_TIMELAPSE_AS_IS or SB_TIMELAPSE_CROP */
+} sb_compositor_opts;
+/* opts NULL: one GPU, no crop, no resize, a panorama.  NULL on failure (sb_last_error): an invalid rig, a blend kind outside
+ * sb_blend_kind (unless timelapse is set), world < 1 or a rank outside [0, world), a crop with a NULL array, only one of
+ * in_w / in_h, a timelapse kind outside sb_timelapse_kind, a timelapse with world > 1, or what the options above refuse. */
+SB_API sb_compositor *sb_compositor_create(const sb_rig *rig, const sb_compositor_opts *opts);
+SB_API void sb_compositor_destroy(sb_compositor *c);
+
 /* Pipelined timelapse step: like sb_compositor_submit, but the step ends in the library's frames.  The library owns
  * 3 x n frames of the canvas in page-locked memory (3 * n * canvas_w * canvas_h * 3 bytes, allocated and zeroed on the first
  * call; SB_ERR_NOMEM names the byte count when they cannot be had, and the next call tries again); only the part of each
@@ -234,10 +241,10 @@ SB_API int sb_compositor_geometry(const sb_compositor *c, int *rects /*[n][4]*/,
 /* compulsory HBM traffic of one run (DESIGN.md byte model) for the roofline: total, and per kernel launch in
  * launch order (same order as sb_compositor_stage_times).  Returns the number of launches (or < 0). */
 SB_API int sb_compositor_model_bytes(const sb_compositor *c, double *total_bytes, double *per_launch, int cap);
-/* host -> device copy of source image i (uint8 HxWx3, the input size with sb_compositor_create_resized); asynchronous on the compositor stream when
+/* host -> device copy of source image i (uint8 HxWx3, in_w[i] x in_h[i] when those are given); asynchronous on the compositor stream when
  * `pinned` != 0 (caller guarantees page-locked memory and keeps it alive until sync) */
 SB_API int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pitch, int pinned);
-/* optional per-image blend mask in warped coordinates (mask_mode 1), uint8 h' x w' */
+/* optional per-image blend mask in warped coordinates, uint8 h' x w'; replaces the warped validity mask from the next run on */
 SB_API int sb_compositor_set_mask(sb_compositor *c, int i, const uint8_t *mask, size_t pitch);
 /* the same from the LOW-resolution seam mask of image i (uint8 sh x sw, what SeamFinder.find returns): the device
  * performs SeamFinder.resize (seam_finder.py:38-43, called at stitcher.py:223-225) -- cv.dilate 3x3, cv.resize to the
@@ -280,12 +287,11 @@ SB_API void sb_host_free(void *p);
  * Multi-GPU (one process per GPU): images are sharded over ranks, each rank composites its shard
  * and the per-band accumulators of overlapping footprints are exchanged with NCCL.
  * ------------------------------------------------------------------------------------------- */
-/* One panorama over `world` GPUs.  Every rank passes the SAME rig (all n images); rank r warps and builds pyramids
+/* One panorama over opts->world GPUs.  Every rank passes the SAME rig (all n images); rank r warps and builds pyramids
  * for images [r*n/world, (r+1)*n/world) only (upload just those) and owns one column strip of the panorama.
  * sb_compositor_run = local kernels + one grouped NCCL send/recv of the per-band partial sums where padded
  * footprints cross strip boundaries + normalise/collapse of the own strip.  Requires sb_comm_init, the
  * multiband blender with >= 1 band and image blocks ordered left to right.  download() returns the strip. */
-SB_API sb_compositor *sb_compositor_create_sharded(const sb_rig *rig, int rank, int world);
 /* first image / number of images of this rank and its output columns [strip[0], strip[1]) in pano-roi coordinates */
 SB_API int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_local, int strip[2]);
 /* 0: `strip` above are columns of the panorama (multiband always; feather when the image blocks lie side by side);

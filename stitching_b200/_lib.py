@@ -40,12 +40,22 @@ class Rig(C.Structure):
         ("src_h", c_int_p),
         ("K", c_float_p),
         ("R", c_float_p),
-        ("mask_mode", C.c_int),
     ]
 
 
 class CropDesc(C.Structure):
     _fields_ = [("rect", c_int_p), ("corner", c_int_p), ("size", c_int_p)]
+
+
+class CompositorOpts(C.Structure):
+    _fields_ = [
+        ("crop", C.POINTER(CropDesc)),
+        ("in_w", c_int_p),
+        ("in_h", c_int_p),
+        ("rank", C.c_int),
+        ("world", C.c_int),
+        ("timelapse", C.c_int),
+    ]
 
 
 # every symbol include/stitch_b200.h declares: (name, restype, argtypes)
@@ -73,7 +83,7 @@ SIGNATURES = [
     ("sb_blender_feed", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_int,
                                   C.c_int, C.c_int]),
     ("sb_blender_blend", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
-    ("sb_compositor_create", C.c_void_p, [C.POINTER(Rig)]),
+    ("sb_compositor_create", C.c_void_p, [C.POINTER(Rig), C.POINTER(CompositorOpts)]),
     ("sb_compositor_destroy", None, [C.c_void_p]),
     ("sb_compositor_geometry", C.c_int, [C.c_void_p, c_int_p, c_int_p, c_int_p]),
     ("sb_compositor_model_bytes", C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int]),
@@ -95,10 +105,6 @@ SIGNATURES = [
     ("sb_compositor_time", C.c_int, [C.c_void_p, C.c_int, C.c_int, c_float_p]),
     ("sb_compositor_time_multi", C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, c_float_p]),
     ("sb_compositor_stage_times", C.c_int, [C.c_void_p, C.POINTER(C.c_char_p), c_float_p, C.c_int]),
-    ("sb_compositor_create_sharded", C.c_void_p, [C.POINTER(Rig), C.c_int, C.c_int]),
-    ("sb_compositor_create_cropped", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), C.c_int, C.c_int]),
-    ("sb_compositor_create_resized", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), c_int_p, c_int_p, C.c_int, C.c_int]),
-    ("sb_compositor_create_timelapse", C.c_void_p, [C.POINTER(Rig), C.POINTER(CropDesc), c_int_p, c_int_p, C.c_int]),
     ("sb_compositor_submit_timelapse", C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(C.c_ulonglong)]),
     ("sb_compositor_timelapse_frame", C.c_int, [C.c_void_p, C.c_ulonglong, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]),
     ("sb_compositor_shard_info", C.c_int, [C.c_void_p, c_int_p, c_int_p, c_int_p]),

@@ -114,30 +114,19 @@ class Compositor:
         self._h = (C.c_int * n)(*[s[1] for s in self.sizes])
         rig = _lib.Rig(n, _lib.WARP_TYPES[warper_type], np.float32(self.scale), _lib.BLEND_KINDS[blender_type],
                        float(blend_strength), self._w, self._h, self._K.ctypes.data_as(_lib.c_float_p),
-                       self._R.ctypes.data_as(_lib.c_float_p), 0)
+                       self._R.ctypes.data_as(_lib.c_float_p))
         L = self._L = _lib.lib()  # close() releases through the library that created the compositor
         self.rank, self.world = int(rank), int(world)
-        desc = None
+        desc = in_w = in_h = None
         if crop is not None:
             arrs = [(C.c_int * (k * n))(*[v for t in ts for v in t]) for k, ts in ((4, crop.rects), (2, crop.corners), (2, crop.sizes))]
-            desc = _lib.CropDesc(*[C.cast(a, _lib.c_int_p) for a in arrs])
-        self.timelapse_kind = timelapse
-        if timelapse is not None:
-            in_w = (C.c_int * n)(*[s[0] for s in self.input_sizes]) if input_sizes is not None else None
-            in_h = (C.c_int * n)(*[s[1] for s in self.input_sizes]) if input_sizes is not None else None
-            self._c = L.sb_compositor_create_timelapse(C.byref(rig), C.byref(desc) if desc is not None else None, in_w, in_h,
-                                                       _lib.TIMELAPSE_KINDS[timelapse])
-        elif input_sizes is not None:
+            desc = C.pointer(_lib.CropDesc(*[C.cast(a, _lib.c_int_p) for a in arrs]))
+        if input_sizes is not None:
             in_w = (C.c_int * n)(*[s[0] for s in self.input_sizes])
             in_h = (C.c_int * n)(*[s[1] for s in self.input_sizes])
-            self._c = L.sb_compositor_create_resized(C.byref(rig), C.byref(desc) if desc is not None else None, in_w, in_h,
-                                                     self.rank, self.world)
-        elif crop is not None:
-            self._c = L.sb_compositor_create_cropped(C.byref(rig), C.byref(desc), self.rank, self.world)
-        elif self.world > 1:
-            self._c = L.sb_compositor_create_sharded(C.byref(rig), self.rank, self.world)
-        else:
-            self._c = L.sb_compositor_create(C.byref(rig))
+        self.timelapse_kind = timelapse
+        opts = _lib.CompositorOpts(desc, in_w, in_h, self.rank, self.world, _lib.TIMELAPSE_KINDS.get(timelapse, 0))
+        self._c = L.sb_compositor_create(C.byref(rig), C.byref(opts))
         if not self._c:
             _lib.check(-1, "sb_compositor_create")
         rects = (C.c_int * (4 * n))()
@@ -243,29 +232,6 @@ class Compositor:
                    "sb_compositor_shard_slab")
         return p.value, n.value
 
-    def submit(self, images, out, out_mask):
-        """Pipelined step: enqueue upload of `images`, warp + blend, download into `out` / `out_mask`; returns a
-        ticket for wait().  At most three tickets in flight; host arrays should live in pinned memory
-        (`pinned_empty`) and must stay untouched until wait(ticket) returns."""
-        n = self.n
-        ptrs = (C.c_void_p * n)()
-        pitches = (C.c_size_t * n)()
-        for i, img in enumerate(images):
-            w, h = self.input_sizes[i]
-            if img.dtype != np.uint8 or img.shape != (h, w, 3) or img.strides[1:] != (3, 1):
-                raise StitchingError(f"image {i}: expected a uint8 {h}x{w}x3 array with packed pixels")
-            ptrs[i] = img.ctypes.data
-            pitches[i] = img.strides[0]
-        ticket = C.c_ulonglong()
-        _lib.check(_lib.lib().sb_compositor_submit(self._c, ptrs, pitches, out.ctypes.data_as(C.c_void_p), out.strides[0],
-                                                   out_mask.ctypes.data_as(C.c_void_p), out_mask.strides[0], C.byref(ticket)),
-                   "sb_compositor_submit")
-        return ticket.value
-
-    def wait(self, ticket):
-        _lib.check(_lib.lib().sb_compositor_wait(self._c, C.c_ulonglong(ticket)), "sb_compositor_wait")
-
-    # -- timelapse (Compositor(..., timelapse="as_is" | "crop")) -------------------------------------------------------
     def _sources(self, images):
         if len(images) != self.n:
             raise StitchingError(f"expected {self.n} images, got {len(images)}")
@@ -279,6 +245,21 @@ class Compositor:
             pitches[i] = img.strides[0]
         return ptrs, pitches
 
+    def submit(self, images, out, out_mask):
+        """Pipelined step: enqueue upload of `images`, warp + blend, download into `out` / `out_mask`; returns a
+        ticket for wait().  At most three tickets in flight; host arrays should live in pinned memory
+        (`pinned_empty`) and must stay untouched until wait(ticket) returns."""
+        ptrs, pitches = self._sources(images)
+        ticket = C.c_ulonglong()
+        _lib.check(_lib.lib().sb_compositor_submit(self._c, ptrs, pitches, out.ctypes.data_as(C.c_void_p), out.strides[0],
+                                                   out_mask.ctypes.data_as(C.c_void_p), out_mask.strides[0], C.byref(ticket)),
+                   "sb_compositor_submit")
+        return ticket.value
+
+    def wait(self, ticket):
+        _lib.check(_lib.lib().sb_compositor_wait(self._c, C.c_ulonglong(ticket)), "sb_compositor_wait")
+
+    # -- timelapse (Compositor(..., timelapse="as_is" | "crop")) -------------------------------------------------------
     def submit_timelapse(self, images):
         """Pipelined timelapse step: enqueue upload of `images`, warp, and the copy of every image's part into its frame;
         returns a ticket for wait() and frames().  At most three tickets in flight; host arrays should live in pinned

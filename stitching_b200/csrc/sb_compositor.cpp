@@ -29,11 +29,11 @@ using namespace sb;
 struct Slot {
     std::vector<uint8_t *> src;    // u8x3 sources as uploaded (null: an image of another rank)
     std::vector<uint32_t *> src4;  // the same, one word per pixel: what the warp kernel reads (repacked after every upload)
-    // An image resized on the device (sb_compositor_create_resized) has its camera-size frame in `src` and its FINAL-size
+    // An image resized on the device (sb_compositor_opts.in_w / in_h) has its camera-size frame in `src` and its FINAL-size
     // source, written by k_resize_src, in `src4` when the warp kernel reads words, else in `fin` (packed u8x3).
     std::vector<uint8_t *> fin;
     PanoOut out{};                 // device outputs
-    // timelapse (sb_compositor_create_timelapse): the pasted parts of the frames, one 16-byte aligned block per image with a
+    // timelapse (sb_compositor_opts.timelapse): the pasted parts of the frames, one 16-byte aligned block per image with a
     // non-empty part; their k_timelapse_paste jobs; the n page-locked frames of the canvas this slot's steps end in
     uint8_t *paste = nullptr;
     PasteJob *paste_jobs = nullptr;
@@ -53,15 +53,15 @@ struct sb_compositor {
     std::vector<char> warp_src4;       // resized images: the warp kernel reads the word-per-pixel source
     std::vector<ResizeJob> resize_jobs;  // scratch of prepare_sources
     std::vector<Rect> rects;           // warped rects (pano-absolute)
-    std::vector<WarpJob> jobs;         // host copy, reading slot 0's sources
-    std::vector<WarpJob> slot_jobs;    // scratch: the jobs of another slot (slot_jobs_of)
+    std::vector<int> warped;           // the images this compositor warps, in launch order (set at creation)
+    std::vector<WarpJob> jobs;         // per image: its warp job without sources (warp_jobs adds a slot's)
+    std::vector<WarpJob> step_jobs;    // scratch of warp_jobs
     bool use_src4 = true;
     std::vector<uint32_t *> rgbm_dev;  // warped, packed; row pitch = width rounded up to 32 pixels (128-byte rows)
     std::vector<float *> tab_dev;
     std::vector<float *> maps_dev;     // projections that are not separable: xmap | ymap of every image (built at plan time)
     std::vector<uint8_t *> usermask_dev;
     std::vector<GainData> gain;        // exposure gains per image (sb_compositor_set_gain)
-    int max_w = 0, max_h = 0;
     BlendPlan plan;
     Slot slots[SB_PIPE_DEPTH];
     int n_slots = 0;                   // slots with buffers: 1 from creation, all from the first submit on
@@ -86,25 +86,20 @@ struct sb_compositor {
     int timelapse = 0;                 // 0, SB_TIMELAPSE_AS_IS or SB_TIMELAPSE_CROP
     Rect canvas{0, 0, 0, 0};           // resultRoi / resultRoiIntersection of the fed rects (pano-absolute)
     std::vector<Rect> part;            // per image: its fed rect on the canvas (P_i, pano-absolute; w = h = 0 when empty)
-    std::vector<int> active;           // the images with a non-empty part, in warp launch order
     std::vector<size_t> paste_off;     // per image: its block in Slot::paste
     size_t paste_bytes = 0;
     long long paste_max = 0;           // largest 3 * |P_i|
     double paste_model = 0;            // model bytes of k_timelapse_paste
-    std::vector<WarpJob> tl_jobs;      // scratch: the jobs of the active images for one slot
 };
 
-static bool is_active(const sb_compositor *c, int i) { return !c->timelapse || c->part[i].w > 0; }
-
-// the sources of this rank's images and an output of slot 0's size (the panorama, or this rank's strip)
+// the sources of the warped images and an output of slot 0's size (the panorama, or this rank's strip)
 static int slot_alloc(sb_compositor *c, Slot &sl)
 {
     cudaStream_t s = c->stream;
     sl.src.assign(c->n, nullptr);
     sl.src4.assign(c->n, nullptr);
     sl.fin.assign(c->n, nullptr);
-    for (int i = c->first; i < c->first + c->count; ++i) {
-        if (!is_active(c, i)) continue;  // an image off the timelapse canvas is neither uploaded nor warped
+    for (int i : c->warped) {
         const long long px = (long long)c->src_w[i] * c->src_h[i];
         if (c->taps_dev[i]) {
             SB_TRY(dev_alloc((void **)&sl.src[i], (size_t)c->in_w[i] * c->in_h[i] * 3 + SB_SRC_PAD, s));
@@ -121,10 +116,10 @@ static int slot_alloc(sb_compositor *c, Slot &sl)
     SB_CUDA(cudaEventCreateWithFlags(&sl.e_comp, cudaEventDisableTiming));
     SB_CUDA(cudaEventCreateWithFlags(&sl.e_d2h, cudaEventDisableTiming));
     if (c->timelapse) {
-        if (c->active.empty()) return SB_OK;
+        if (c->warped.empty()) return SB_OK;
         SB_TRY(dev_alloc((void **)&sl.paste, c->paste_bytes, s));
         std::vector<PasteJob> pj;
-        for (int i : c->active)
+        for (int i : c->warped)
             pj.push_back(PasteJob{c->rgbm_dev[i], sl.paste + c->paste_off[i], rgbm_pitch_of(c->part[i].w), c->part[i].w, c->part[i].h});
         SB_TRY(dev_alloc((void **)&sl.paste_jobs, pj.size() * sizeof(PasteJob), s));
         SB_CUDA(cudaMemcpyAsync(sl.paste_jobs, pj.data(), pj.size() * sizeof(PasteJob), cudaMemcpyHostToDevice, s));
@@ -246,14 +241,13 @@ static int check_input_sizes(const sb_rig *rig, const int *in_w, const int *in_h
     return SB_OK;
 }
 
-// The taps of the resized images of this rank, and which source layout their warp kernel reads: launch_warp chooses
+// The taps of the resized warped images, and which source layout their warp kernel reads: launch_warp chooses
 // its kernel per batch of SB_WARP_BATCH jobs, and reads the word-per-pixel sources only when the RGBM kernel runs and
 // every job of the batch has one (slot_alloc's rule); a resized image gets only the buffer that is read.
 static int plan_resize(sb_compositor *c, cudaStream_t s)
 {
-    std::vector<int> t, order = c->active;  // the images in launch order: a timelapse warps only those on its canvas
-    if (!c->timelapse)
-        for (int i = c->first; i < c->first + c->count; ++i) order.push_back(i);
+    std::vector<int> t;
+    const std::vector<int> &order = c->warped;
     std::vector<WarpJob> batch;
     for (size_t b = 0; b < order.size(); b += SB_WARP_BATCH) {
         const size_t end = std::min(b + SB_WARP_BATCH, order.size());
@@ -336,7 +330,6 @@ static int plan_timelapse(sb_compositor *c, int kind, const int *corners, const 
         if (x1 <= x0 || y1 <= y0) continue;
         c->part[i] = Rect{x0, y0, x1 - x0, y1 - y0};
         proj[i] = Rect{proj[i].x + x0 - r.x, proj[i].y + y0 - r.y, x1 - x0, y1 - y0};
-        c->active.push_back(i);
         const long long bytes = 3ll * (x1 - x0) * (y1 - y0);
         c->paste_off[i] = c->paste_bytes;
         c->paste_bytes += ((size_t)bytes + 15) & ~(size_t)15;
@@ -346,19 +339,18 @@ static int plan_timelapse(sb_compositor *c, int kind, const int *corners, const 
     return SB_OK;
 }
 
-// in_w / in_h: null, or the size of the frame of every image (sb_compositor_create_resized); timelapse: 0 or a
-// sb_timelapse_kind (sb_compositor_create_timelapse)
-static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h, int rank,
-                            int world, int timelapse)
+// `o` has passed valid_opts
+static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_compositor_opts &o)
 {
-    c->timelapse = timelapse;
+    const int *in_w = o.in_w, *in_h = o.in_h;
+    const sb_crop *crop = o.crop;
+    c->timelapse = o.timelapse;
     const int n = rig->n_images;
     c->n = n;
-    c->sharded = world > 1;
+    c->sharded = o.world > 1;
     c->first = 0;
     c->count = n;
-    if (c->sharded) ShardPlan::block_of(n, world, rank, &c->first, &c->count);
-    auto mine = [&](int i) { return i >= c->first && i < c->first + c->count; };
+    if (c->sharded) ShardPlan::block_of(n, o.world, o.rank, &c->first, &c->count);
     SB_TRY(ensure_device());
     SB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     cudaStream_t s = c->stream;
@@ -416,14 +408,14 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *
         }
         proj[i] = Rect{rect[0], rect[1], rect[2], rect[3]};
     }
-    if (timelapse) SB_TRY(plan_timelapse(c, timelapse, corners.data(), sizes.data(), proj.data()));
+    if (c->timelapse) SB_TRY(plan_timelapse(c, c->timelapse, corners.data(), sizes.data(), proj.data()));
+    // the images this compositor warps: its block, less those off the timelapse canvas (neither uploaded nor warped)
+    for (int i = c->first; i < c->first + c->count; ++i)
+        if (!c->timelapse || c->part[i].w > 0) c->warped.push_back(i);
     std::vector<float> host_tab;
-    for (int i = 0; i < n; ++i) {
+    for (int i : c->warped) {
         const Projector &p = projs[i];
         int rect[4] = {proj[i].x, proj[i].y, proj[i].w, proj[i].h};
-        c->max_w = std::max(c->max_w, rect[2]);
-        c->max_h = std::max(c->max_h, rect[3]);
-        if (!mine(i) || !is_active(c, i)) continue;  // another rank warps this image, or it is off the timelapse canvas
         SB_TRY(dev_alloc((void **)&c->rgbm_dev[i], (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
         // the row padding (never written by the warp kernel) is read by the tile kernels' 16-byte copies: weight 0
         SB_CUDA(cudaMemsetAsync(c->rgbm_dev[i], 0, (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
@@ -439,78 +431,66 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_crop *
         c->jobs[i].rgbm_pitch = rgbm_pitch_of(rect[2]);
         c->warp_bytes += 3.0 * c->src_w[i] * c->src_h[i] + 4.0 * rect[2] * rect[3];
     }
-    if (timelapse) {
-        // no blend plan: the step is warp -> paste into this slot's frames
-        SB_TRY(plan_resize(c, s));
-        SB_TRY(slot_alloc(c, c->slots[0]));
-        c->n_slots = 1;
-        for (int i : c->active) {
-            c->jobs[i].src = warp_src(c, c->slots[0], i);
-            c->jobs[i].src4 = c->slots[0].src4[i];
+    if (!c->timelapse) {  // a timelapse has no blend plan: its step is warp -> paste into the slot's frames
+        // Blender.prepare (blender.py:23-38)
+        const Rect roi = result_roi(corners.data(), sizes.data(), n);
+        int kind, nbr;
+        float sharp;
+        derive_blend_params(rig->blend_kind, rig->blend_strength, roi, &kind, &nbr, &sharp);
+        SB_TRY(c->plan.set_geometry(kind, nbr, sharp, roi));
+        {
+            // the mask byte of a warped pixel is the validity test's 0 / 255 until a caller supplies masks (SB_PD_BIN=0: A/B switch)
+            const char *e = getenv("SB_PD_BIN");
+            c->plan.binary_masks = !(e && e[0] == '0');
         }
-        SB_CUDA(cudaStreamSynchronize(s));
-        return SB_OK;
+        for (int i = 0; i < n; ++i) {
+            FeedDesc f;
+            std::memset(&f, 0, sizeof f);
+            f.w = c->rects[i].w;
+            f.h = c->rects[i].h;
+            f.tlx = c->rects[i].x;
+            f.tly = c->rects[i].y;
+            f.rgbm = c->rgbm_dev[i];
+            f.rgbm_pitch = rgbm_pitch_of(c->rects[i].w);
+            SB_TRY(c->plan.add_feed(f));
+        }
+        int out_w = roi.w, out_h = roi.h;
+        if (c->sharded) {
+            c->plan.active_first = c->first;
+            c->plan.active_count = c->count;
+            SB_TRY(c->shard.build(c->plan, o.rank, o.world));
+            int lo, hi;
+            c->shard.strip(c->plan, &lo, &hi);
+            if (c->shard.axis == 0)
+                out_w = hi - lo;
+            else
+                out_h = hi - lo;  // row strips (feather, image blocks stacked vertically)
+        }
+        SB_TRY(c->plan.allocate(s));
+        if (c->sharded) SB_TRY(c->shard.allocate(c->plan, s));
+        c->slots[0].out.w = out_w;
+        c->slots[0].out.h = out_h;
     }
-
-    // Blender.prepare (blender.py:23-38)
-    const Rect roi = result_roi(corners.data(), sizes.data(), n);
-    int kind, nbr;
-    float sharp;
-    derive_blend_params(rig->blend_kind, rig->blend_strength, roi, &kind, &nbr, &sharp);
-    SB_TRY(c->plan.set_geometry(kind, nbr, sharp, roi));
-    {
-        // the mask byte of a warped pixel is the validity test's 0 / 255 until a caller supplies masks (SB_PD_BIN=0: A/B switch)
-        const char *e = getenv("SB_PD_BIN");
-        c->plan.binary_masks = !(e && e[0] == '0');
-    }
-    for (int i = 0; i < n; ++i) {
-        FeedDesc f;
-        std::memset(&f, 0, sizeof f);
-        f.w = c->rects[i].w;
-        f.h = c->rects[i].h;
-        f.tlx = c->rects[i].x;
-        f.tly = c->rects[i].y;
-        f.rgbm = c->rgbm_dev[i];
-        f.rgbm_pitch = rgbm_pitch_of(c->rects[i].w);
-        SB_TRY(c->plan.add_feed(f));
-    }
-    int out_w = roi.w, out_h = roi.h;
-    if (c->sharded) {
-        c->plan.active_first = c->first;
-        c->plan.active_count = c->count;
-        SB_TRY(c->shard.build(c->plan, rank, world));
-        int lo, hi;
-        c->shard.strip(c->plan, &lo, &hi);
-        if (c->shard.axis == 0)
-            out_w = hi - lo;
-        else
-            out_h = hi - lo;  // row strips (feather, image blocks stacked vertically)
-    }
-    SB_TRY(c->plan.allocate(s));
-    if (c->sharded) SB_TRY(c->shard.allocate(c->plan, s));
     SB_TRY(plan_resize(c, s));
-    c->slots[0].out.w = out_w;
-    c->slots[0].out.h = out_h;
     SB_TRY(slot_alloc(c, c->slots[0]));
     c->n_slots = 1;
-    for (int i = c->first; i < c->first + c->count; ++i) {
-        c->jobs[i].src = warp_src(c, c->slots[0], i);
-        c->jobs[i].src4 = c->slots[0].src4[i];
-    }
     SB_CUDA(cudaStreamSynchronize(s));
     return SB_OK;
 }
 
-// the jobs of `slot`: `jobs` with the slot's sources swapped in (built in a scratch vector: no allocation per step)
-static const WarpJob *slot_jobs_of(sb_compositor *c, int slot)
+// the warp jobs of one step on `slot`: those of the warped images, in launch order, with the slot's sources (built in a
+// scratch vector: no allocation per step); c->warped.size() of them
+static const WarpJob *warp_jobs(sb_compositor *c, int slot)
 {
-    if (slot == 0) return c->jobs.data();
-    c->slot_jobs = c->jobs;
-    for (int i = 0; i < c->n; ++i) {
-        c->slot_jobs[i].src = warp_src(c, c->slots[slot], i);
-        c->slot_jobs[i].src4 = c->slots[slot].src4[i];
+    const Slot &sl = c->slots[slot];
+    c->step_jobs.clear();
+    for (int i : c->warped) {
+        WarpJob j = c->jobs[i];
+        j.src = warp_src(c, sl, i);
+        j.src4 = sl.src4[i];
+        c->step_jobs.push_back(j);
     }
-    return c->slot_jobs.data();
+    return c->step_jobs.data();
 }
 
 // the jobs are baked into the captured steps: capture again on next use
@@ -619,19 +599,6 @@ static int shard_local(sb_compositor *c, cudaStream_t s, const std::function<int
     return SB_OK;
 }
 
-// the jobs of the images on the timelapse canvas with `slot`'s sources (built in a scratch vector)
-static const WarpJob *timelapse_jobs_of(sb_compositor *c, int slot)
-{
-    c->tl_jobs.clear();
-    for (int i : c->active) {
-        WarpJob j = c->jobs[i];
-        j.src = warp_src(c, c->slots[slot], i);
-        j.src4 = c->slots[slot].src4[i];
-        c->tl_jobs.push_back(j);
-    }
-    return c->tl_jobs.data();
-}
-
 static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
 {
     cudaStream_t s = c->stream;
@@ -651,15 +618,12 @@ static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
         return SB_OK;
     };
     SB_TRY(mark("start"));
+    SB_TRY(launch_warp(warp_jobs(c, slot), (int)c->warped.size(), s));
+    SB_TRY(mark("warp"));
     if (c->timelapse) {
-        const int na = (int)c->active.size();
-        SB_TRY(launch_warp(timelapse_jobs_of(c, slot), na, s));
-        SB_TRY(mark("warp"));
-        SB_TRY(launch_timelapse_paste(c->slots[slot].paste_jobs, na, c->paste_max, s));
+        SB_TRY(launch_timelapse_paste(c->slots[slot].paste_jobs, (int)c->warped.size(), c->paste_max, s));
         return mark("paste");
     }
-    SB_TRY(launch_warp(slot_jobs_of(c, slot) + c->first, c->count, s));
-    SB_TRY(mark("warp"));
     const PanoOut &out = c->slots[slot].out;
     if (!c->sharded) return c->plan.run(out, s, events ? std::function<int(const std::string &)>(mark) : nullptr);
     if (!c->comm_stream) {
@@ -808,12 +772,71 @@ static int compositor_pipe_init(sb_compositor *c)
     return SB_OK;
 }
 
+// One pipelined step of sb_compositor_submit / _submit_timelapse (`what`) on the next slot: H2D of the warped images,
+// the step, and `download`'s D2H of the slot's output are enqueued on three streams and chained with events; with three
+// buffer sets the copies of a step overlap the kernels and copies of its neighbours.
+static int pipe_step(sb_compositor *c, const char *what, const uint8_t *const *srcs, const size_t *pitches,
+                     const std::function<int(const Slot &)> &download, unsigned long long *ticket)
+{
+    for (int i = 0; i < c->n; ++i)
+        if (!srcs[i] || pitches[i] < (size_t)c->in_w[i] * 3) {
+            set_error("%s: invalid source %d", what, i);
+            return SB_ERR_INVALID;
+        }
+    if (!pipe_ready(c)) SB_TRY(compositor_pipe_init(c));
+    const unsigned long long t = c->submitted;
+    const int slot = (int)(t % SB_PIPE_DEPTH);
+    Slot &sl = c->slots[slot];
+    // sources of this slot are free once the previous compute that read them has finished; on a slot's first use
+    // that is whatever upload() / run() / sb_compositor_time() queued on the compute stream before this submit
+    // (download() is synchronous, so the output buffers need no such guard)
+    if (t < SB_PIPE_DEPTH) SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
+    SB_CUDA(cudaStreamWaitEvent(c->h2d, sl.e_comp, 0));
+    for (int i : c->warped)
+        SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->in_w[i] * 3, srcs[i], pitches[i], (size_t)c->in_w[i] * 3, c->in_h[i],
+                          cudaMemcpyHostToDevice, c->h2d));
+    // the repack (and resize) kernels follow the LAST copy (same stream): a kernel between two copies would leave the PCIe
+    // link idle for its launch + run time, eight times per step
+    SB_TRY(prepare_sources(c, sl, 0, c->n, c->h2d));
+    SB_CUDA(cudaEventRecord(sl.e_h2d, c->h2d));
+    SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_h2d, 0));
+    // the output buffers of this slot (panorama or pasted parts) are free once their previous download has finished
+    if (t >= SB_PIPE_DEPTH) SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_d2h, 0));
+    SB_TRY(compositor_enqueue(c, false, slot));
+    SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
+    SB_CUDA(cudaStreamWaitEvent(c->d2h, sl.e_comp, 0));
+    SB_TRY(download(sl));
+    SB_CUDA(cudaEventRecord(sl.e_d2h, c->d2h));
+    c->submitted = t + 1;
+    if (ticket) *ticket = t;
+    return SB_OK;
+}
+
 // blend: false when the rig's blend fields are unused (a timelapse compositor)
 static bool valid_rig(const sb_rig *rig, bool blend = true)
 {
     return rig && rig->n_images > 0 && rig->n_images <= SB_MAX_IMAGES && rig->src_w && rig->src_h && rig->K && rig->R &&
            rig->warp_type >= SB_WARP_SPHERICAL && rig->warp_type <= SB_WARP_TRANSVERSE_MERCATOR &&
            (!blend || (rig->blend_kind >= SB_BLEND_NO && rig->blend_kind <= SB_BLEND_MULTIBAND));
+}
+
+// what sb_compositor_create refuses before it builds anything
+static bool valid_opts(const sb_rig *rig, const sb_compositor_opts &o)
+{
+    if (o.timelapse && o.timelapse != SB_TIMELAPSE_AS_IS && o.timelapse != SB_TIMELAPSE_CROP) {
+        set_error("sb_compositor_create: unknown timelapse kind %d", o.timelapse);
+        return false;
+    }
+    if (!valid_rig(rig, !o.timelapse) || o.world < 1 || o.rank < 0 || o.rank >= o.world || !o.in_w != !o.in_h ||
+        (o.crop && (!o.crop->rect || !o.crop->corner || !o.crop->size))) {
+        set_error("sb_compositor_create: invalid argument");
+        return false;
+    }
+    if (o.timelapse && o.world > 1) {
+        set_error("sb_compositor_create: invalid argument: a timelapse compositor runs on one GPU, not %d", o.world);
+        return false;
+    }
+    return true;
 }
 
 // the entries that need a panorama, warped images, masks or a shard: a timelapse compositor has none of them
@@ -824,74 +847,18 @@ static bool refuse_timelapse(const sb_compositor *c, const char *what)
     return true;
 }
 
-static sb_compositor *compositor_create(const sb_rig *rig, const sb_crop *crop, int rank, int world, const int *in_w = nullptr,
-                                        const int *in_h = nullptr, int timelapse = 0)
+extern "C" {
+
+sb_compositor *sb_compositor_create(const sb_rig *rig, const sb_compositor_opts *opts)
 {
+    const sb_compositor_opts o = opts ? *opts : sb_compositor_opts{nullptr, nullptr, nullptr, 0, 1, 0};
+    if (!valid_opts(rig, o)) return nullptr;
     sb_compositor *c = new sb_compositor;
-    if (compositor_build(c, rig, crop, in_w, in_h, rank, world, timelapse) != SB_OK) {
+    if (compositor_build(c, rig, o) != SB_OK) {
         compositor_free(c);
         return nullptr;
     }
     return c;
-}
-
-extern "C" {
-
-sb_compositor *sb_compositor_create(const sb_rig *rig)
-{
-    if (!valid_rig(rig)) {
-        set_error("sb_compositor_create: invalid rig");
-        return nullptr;
-    }
-    return compositor_create(rig, nullptr, 0, 1);
-}
-
-// One panorama over `world` GPUs (one process each): this rank warps and pyramids images
-// [rank*n/world, (rank+1)*n/world) and owns one column strip of the panorama (sb_shard.h).
-sb_compositor *sb_compositor_create_sharded(const sb_rig *rig, int rank, int world)
-{
-    if (!valid_rig(rig) || world < 1 || rank < 0 || rank >= world) {
-        set_error("sb_compositor_create_sharded: invalid argument");
-        return nullptr;
-    }
-    return compositor_create(rig, nullptr, rank, world);
-}
-
-// Either of the two above, with every image cropped as Stitcher.crop_final_resolution does (crop_image)
-sb_compositor *sb_compositor_create_cropped(const sb_rig *rig, const sb_crop *crop, int rank, int world)
-{
-    if (!valid_rig(rig) || world < 1 || rank < 0 || rank >= world || (crop && (!crop->rect || !crop->corner || !crop->size))) {
-        set_error("sb_compositor_create_cropped: invalid argument");
-        return nullptr;
-    }
-    return compositor_create(rig, crop, rank, world);
-}
-
-// Any of the above taking camera-size frames: image i is uploaded / submitted at in_w[i] x in_h[i] and resized on the
-// device to its FINAL size rig->src_w[i] x rig->src_h[i] (Images.resize_img_by_scaler), or taken as it is when the two
-// sizes are equal
-sb_compositor *sb_compositor_create_resized(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h, int rank, int world)
-{
-    if (!valid_rig(rig) || !in_w || !in_h || world < 1 || rank < 0 || rank >= world || (crop && (!crop->rect || !crop->corner || !crop->size))) {
-        set_error("sb_compositor_create_resized: invalid argument");
-        return nullptr;
-    }
-    return compositor_create(rig, crop, rank, world, in_w, in_h);
-}
-
-// Stitcher with timelapse="as_is" / "crop" (stitcher.py:241-252): one GPU, every step writes one frame per image
-// (plan_timelapse); crop and in_w / in_h as in sb_compositor_create_resized, both nullable
-sb_compositor *sb_compositor_create_timelapse(const sb_rig *rig, const sb_crop *crop, const int *in_w, const int *in_h, int kind)
-{
-    if (kind != SB_TIMELAPSE_AS_IS && kind != SB_TIMELAPSE_CROP) {
-        set_error("sb_compositor_create_timelapse: unknown timelapse kind %d", kind);
-        return nullptr;
-    }
-    if (!valid_rig(rig, false) || !in_w != !in_h || (crop && (!crop->rect || !crop->corner || !crop->size))) {
-        set_error("sb_compositor_create_timelapse: invalid argument");
-        return nullptr;
-    }
-    return compositor_create(rig, crop, 0, 1, in_w, in_h, kind);
 }
 
 int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_local, int strip[2])
@@ -922,7 +889,7 @@ int sb_compositor_shard_phase(sb_compositor *c, int phase)
     cudaStream_t s = c->stream;
     auto nomark = [](const std::string &) -> int { return SB_OK; };
     if (phase == 0) {
-        SB_TRY(launch_warp(c->jobs.data() + c->first, c->count, s));
+        SB_TRY(launch_warp(warp_jobs(c, 0), (int)c->warped.size(), s));
         SB_TRY(shard_local(c, s, std::function<int(const std::string &)>(nomark)));
     } else if (c->plan.kind == SB_BLEND_FEATHER) {
         SB_TRY(c->shard.feather_finish(c->plan, c->slots[0].out, s));
@@ -1054,7 +1021,7 @@ int sb_compositor_set_gain(sb_compositor *c, int i, const float *gain_map, int g
         set_error("sb_compositor_set_gain: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
     }
-    if (!is_active(c, i)) return SB_OK;  // off the timelapse canvas: nothing of it is shown
+    if (!c->rgbm_dev[i]) return SB_OK;  // off the timelapse canvas: nothing of it is shown
     // ExposureErrorCompensator.apply(i, corner, warped image, mask) (exposure_error_compensator.py:43-45,
     // stitcher.py:219-221) fused into the warp's epilogue: the warped image never exists uncompensated
     SB_CUDA(cudaStreamSynchronize(c->stream));  // the previous run may still read the old gain buffers
@@ -1098,8 +1065,7 @@ int sb_compositor_download(sb_compositor *c, uint8_t *dst, size_t dst_pitch, uin
     return SB_OK;
 }
 
-// Pipelined end-to-end step: H2D of this batch, warp + blend, D2H of the panorama are enqueued on three
-// streams and chained with events; with three buffer sets the copies of a step overlap the kernels and copies of its neighbours.
+// Pipelined end-to-end step: the D2H of the panorama ends it (pipe_step).
 int sb_compositor_submit(sb_compositor *c, const uint8_t *const *srcs, const size_t *pitches, uint8_t *dst, size_t dst_pitch,
                          uint8_t *dst_mask, size_t mask_pitch, unsigned long long *ticket)
 {
@@ -1112,38 +1078,8 @@ int sb_compositor_submit(sb_compositor *c, const uint8_t *const *srcs, const siz
         set_error("sb_compositor_submit: the pipelined path is single-GPU; use upload / run / download on a sharded compositor");
         return SB_ERR_STATE;
     }
-    for (int i = 0; i < c->n; ++i)
-        if (!srcs[i] || pitches[i] < (size_t)c->in_w[i] * 3) {
-            set_error("sb_compositor_submit: invalid source %d", i);
-            return SB_ERR_INVALID;
-        }
-    if (c->n_slots < SB_PIPE_DEPTH) SB_TRY(compositor_pipe_init(c));
-    const unsigned long long t = c->submitted;
-    const int slot = (int)(t % SB_PIPE_DEPTH);
-    Slot &sl = c->slots[slot];
-    // sources of this slot are free once the previous compute that read them has finished; on a slot's first use
-    // that is whatever upload() / run() / sb_compositor_time() queued on the compute stream before this submit
-    // (download() is synchronous, so the output buffers need no such guard)
-    if (t < SB_PIPE_DEPTH) SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
-    SB_CUDA(cudaStreamWaitEvent(c->h2d, sl.e_comp, 0));
-    for (int i = 0; i < c->n; ++i)
-        SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->in_w[i] * 3, srcs[i], pitches[i], (size_t)c->in_w[i] * 3, c->in_h[i],
-                                  cudaMemcpyHostToDevice, c->h2d));
-    // the repack (and resize) kernels follow the LAST copy (same stream): a kernel between two copies would leave the PCIe
-    // link idle for its launch + run time, eight times per step
-    SB_TRY(prepare_sources(c, sl, 0, c->n, c->h2d));
-    SB_CUDA(cudaEventRecord(sl.e_h2d, c->h2d));
-    SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_h2d, 0));
-    // the output buffers of this slot are free once their previous download has finished
-    if (t >= SB_PIPE_DEPTH) SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_d2h, 0));
-    SB_TRY(compositor_enqueue(c, false, slot));
-    SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
-    SB_CUDA(cudaStreamWaitEvent(c->d2h, sl.e_comp, 0));
-    SB_TRY(download_out(sl.out, dst, dst_pitch, dst_mask, mask_pitch, c->d2h));
-    SB_CUDA(cudaEventRecord(sl.e_d2h, c->d2h));
-    c->submitted = t + 1;
-    if (ticket) *ticket = t;
-    return SB_OK;
+    auto download = [&](const Slot &sl) { return download_out(sl.out, dst, dst_pitch, dst_mask, mask_pitch, c->d2h); };
+    return pipe_step(c, "sb_compositor_submit", srcs, pitches, download, ticket);
 }
 
 int sb_compositor_wait(sb_compositor *c, unsigned long long ticket)
@@ -1165,43 +1101,20 @@ int sb_compositor_submit_timelapse(sb_compositor *c, const uint8_t *const *srcs,
         return SB_ERR_INVALID;
     }
     if (!c->timelapse) {
-        set_error("sb_compositor_submit_timelapse: not a timelapse compositor (sb_compositor_create_timelapse)");
+        set_error("sb_compositor_submit_timelapse: not a timelapse compositor (sb_compositor_opts.timelapse)");
         return SB_ERR_STATE;
     }
-    for (int i = 0; i < c->n; ++i)
-        if (!srcs[i] || pitches[i] < (size_t)c->in_w[i] * 3) {
-            set_error("sb_compositor_submit_timelapse: invalid source %d", i);
-            return SB_ERR_INVALID;
+    auto download = [c](const Slot &sl) -> int {
+        const Rect &cv = c->canvas;
+        const size_t fpitch = (size_t)cv.w * 3, fbytes = fpitch * cv.h;
+        for (int i : c->warped) {
+            const Rect &p = c->part[i];
+            uint8_t *dst = sl.frames + fbytes * i + (size_t)(p.y - cv.y) * fpitch + (size_t)(p.x - cv.x) * 3;
+            SB_CUDA(sb_copy2d(dst, fpitch, sl.paste + c->paste_off[i], (size_t)p.w * 3, (size_t)p.w * 3, p.h, cudaMemcpyDeviceToHost, c->d2h));
         }
-    if (!pipe_ready(c)) SB_TRY(compositor_pipe_init(c));
-    const unsigned long long t = c->submitted;
-    const int slot = (int)(t % SB_PIPE_DEPTH);
-    Slot &sl = c->slots[slot];
-    // as in sb_compositor_submit: the sources are free once the previous compute that read them has finished
-    if (t < SB_PIPE_DEPTH) SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
-    SB_CUDA(cudaStreamWaitEvent(c->h2d, sl.e_comp, 0));
-    for (int i : c->active)
-        SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->in_w[i] * 3, srcs[i], pitches[i], (size_t)c->in_w[i] * 3, c->in_h[i],
-                          cudaMemcpyHostToDevice, c->h2d));
-    SB_TRY(prepare_sources(c, sl, 0, c->n, c->h2d));
-    SB_CUDA(cudaEventRecord(sl.e_h2d, c->h2d));
-    SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_h2d, 0));
-    // the paste buffer of this slot is free once its previous download has finished
-    if (t >= SB_PIPE_DEPTH) SB_CUDA(cudaStreamWaitEvent(c->stream, sl.e_d2h, 0));
-    SB_TRY(compositor_enqueue(c, false, slot));
-    SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
-    SB_CUDA(cudaStreamWaitEvent(c->d2h, sl.e_comp, 0));
-    const Rect &cv = c->canvas;
-    const size_t fpitch = (size_t)cv.w * 3, fbytes = fpitch * cv.h;
-    for (int i : c->active) {
-        const Rect &p = c->part[i];
-        uint8_t *dst = sl.frames + fbytes * i + (size_t)(p.y - cv.y) * fpitch + (size_t)(p.x - cv.x) * 3;
-        SB_CUDA(sb_copy2d(dst, fpitch, sl.paste + c->paste_off[i], (size_t)p.w * 3, (size_t)p.w * 3, p.h, cudaMemcpyDeviceToHost, c->d2h));
-    }
-    SB_CUDA(cudaEventRecord(sl.e_d2h, c->d2h));
-    c->submitted = t + 1;
-    if (ticket) *ticket = t;
-    return SB_OK;
+        return SB_OK;
+    };
+    return pipe_step(c, "sb_compositor_submit_timelapse", srcs, pitches, download, ticket);
 }
 
 int sb_compositor_timelapse_frame(const sb_compositor *c, unsigned long long ticket, int i, const uint8_t **frame, size_t *pitch)
@@ -1320,7 +1233,6 @@ int sb_compositor_time(sb_compositor *c, int iters, int flush_l2, float *ms_tota
     *ms_total = total;
     // pass 2: per-kernel breakdown (individual launches with an event after each), a few iterations
     iters = iters < 5 ? iters : 5;
-    total = 0.f;
     c->launch_ms.clear();
     for (int it = 0; it < iters; ++it) {
         if (flush_l2) SB_TRY(launch_flush_l2(c->flush_buf, c->flush_bytes, s));
@@ -1333,9 +1245,6 @@ int sb_compositor_time(sb_compositor *c, int iters, int flush_l2, float *ms_tota
             SB_CUDA(cudaEventElapsedTime(&t, c->ev[k], c->ev[k + 1]));
             c->launch_ms[k] += t;
         }
-        float t = 0;
-        SB_CUDA(cudaEventElapsedTime(&t, c->ev[0], c->ev[nl]));
-        total += t;
     }
     for (float &v : c->launch_ms) v /= (float)iters;
     return SB_OK;

@@ -222,7 +222,7 @@ int launch_repack_rgbx(const uint8_t *rgb, uint32_t *dst, long long pixels, cuda
 // launch_warp's kernel choice for a batch of jobs: true when it reads WarpJob::src4 of jobs that have one (sb_warp.cu)
 bool warp_batch_rgbm(const WarpJob *jobs, int cnt);
 // one image of k_resize_src: Images.resize_img_by_scaler (cv.resize INTER_LINEAR_EXACT) from a camera-size frame into
-// the warp's source layout, in place of the repack (sb_compositor_create_resized)
+// the warp's source layout, in place of the repack (sb_compositor_opts.in_w / in_h)
 struct ResizeJob {
     const uint8_t *src;  // camera-size u8x3, rows of 3 * sw bytes, SB_SRC_PAD spare bytes after the last
     uint32_t *dst4;      // FINAL size, one word per pixel (WarpJob::src4), or null:

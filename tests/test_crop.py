@@ -1,5 +1,5 @@
 """The compositor with a crop (Stitcher's default Cropper), in the emulation build: bit for bit against the oracle that
-slices the warped images as Stitcher.crop_final_resolution does, and the refusals of sb_compositor_create_cropped."""
+slices the warped images as Stitcher.crop_final_resolution does, and the refusals of a cropped sb_compositor_create."""
 import os
 import types
 

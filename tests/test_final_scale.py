@@ -141,6 +141,8 @@ def test_refusals(use_emu):
             c.upload(imgs)  # the FINAL-size frame where the camera frame belongs
         with pytest.raises(StitchingError, match="image 0: expected a uint8"):
             c.submit(imgs, np.empty((1, 1, 3), np.uint8), np.empty((1, 1), np.uint8))
+        with pytest.raises(StitchingError, match=f"expected {case.n} images"):
+            c.submit(imgs[1:], np.empty((1, 1, 3), np.uint8), np.empty((1, 1), np.uint8))
         with pytest.raises(StitchingError, match="image 0: expected uint8"):
             c.composite(imgs)
     finally:

@@ -113,7 +113,8 @@ def test_sharded_rejects_what_it_cannot_do(use_emu):
 
 
 def test_sharded_create_rejects_an_unknown_blend_kind(use_emu):
-    """Both creates check the rig alike: a blend kind outside sb_blend_kind is refused, not built as a feather blend."""
+    """A sharded create checks the rig like a single-GPU one: a blend kind outside sb_blend_kind is refused, not built as
+    a feather blend."""
     from stitching_b200 import Warper, _lib
 
     cams = rigs.yaw_ring(4, 64, 48, 70, 25)  # blocks run left to right: a feather blend of this rig can be sharded
@@ -121,15 +122,15 @@ def test_sharded_create_rejects_an_unknown_blend_kind(use_emu):
     R = np.ascontiguousarray(np.stack([cam.R for cam in cams]).astype(np.float32))
     w, h = (C.c_int * 4)(*[64] * 4), (C.c_int * 4)(*[48] * 4)
 
-    def create_sharded(kind):
+    def create(kind):
         rig = _lib.Rig(4, _lib.WARP_TYPES["spherical"], 70.0, kind, 5.0, w, h, K.ctypes.data_as(_lib.c_float_p),
-                       R.ctypes.data_as(_lib.c_float_p), 0)
-        return use_emu.sb_compositor_create_sharded(C.byref(rig), 0, 2)
+                       R.ctypes.data_as(_lib.c_float_p))
+        return use_emu.sb_compositor_create(C.byref(rig), C.byref(_lib.CompositorOpts(rank=0, world=2)))
 
-    c = create_sharded(_lib.BLEND_KINDS["feather"])
+    c = create(_lib.BLEND_KINDS["feather"])
     assert c
     use_emu.sb_compositor_destroy(c)
-    assert not create_sharded(7)
+    assert not create(7)
     assert b"invalid" in use_emu.sb_last_error()
 
 

@@ -158,13 +158,17 @@ def test_refusals(use_emu):
         Compositor(case.cams, case.sizes, case.wtype, timelapse="no")
     with pytest.raises(StitchingError, match="one GPU"):
         Compositor(case.cams, case.sizes, case.wtype, timelapse="crop", rank=0, world=2)
-    # the C ABI refuses a kind outside the enum
-    rig = _lib.Rig(case.n, 0, 1.0, 0, 5.0, (ctypes.c_int * case.n)(*[s[0] for s in case.sizes]),
-                   (ctypes.c_int * case.n)(*[s[1] for s in case.sizes]), (ctypes.c_float * (9 * case.n))(),
-                   (ctypes.c_float * (9 * case.n))(), 0)
-    for kind in (0, 3):
-        assert not L.sb_compositor_create_timelapse(ctypes.byref(rig), None, None, None, kind)
+    # the C ABI refuses a kind outside the enum, a timelapse over two GPUs and in_w without in_h
+    w = (ctypes.c_int * case.n)(*[s[0] for s in case.sizes])
+    rig = _lib.Rig(case.n, 0, 1.0, 0, 5.0, w, (ctypes.c_int * case.n)(*[s[1] for s in case.sizes]),
+                   (ctypes.c_float * (9 * case.n))(), (ctypes.c_float * (9 * case.n))())
+    for kind in (3, -1):
+        assert not L.sb_compositor_create(ctypes.byref(rig), ctypes.byref(_lib.CompositorOpts(world=1, timelapse=kind)))
         assert b"unknown timelapse kind" in L.sb_last_error()
+    assert not L.sb_compositor_create(ctypes.byref(rig), ctypes.byref(_lib.CompositorOpts(rank=0, world=2, timelapse=1)))
+    assert b"one GPU" in L.sb_last_error()
+    assert not L.sb_compositor_create(ctypes.byref(rig), ctypes.byref(_lib.CompositorOpts(in_w=w, world=1, timelapse=1)))
+    assert b"invalid argument" in L.sb_last_error()
 
 
 def test_frames_out_of_pinned_memory(use_emu, oracle, monkeypatch):
