@@ -8,15 +8,18 @@
 // What changed against k_collapse_fast is where the operands come from and how often they are touched.  The profile of
 // k_collapse_fast shows 845 warp instructions per quad at level 0: 340 in the final pyrUp +
 // store, ~190 per covering image, mostly address arithmetic, bounds tests and 9 + 27 scattered global taps per thread.
-// Here a CTA owns a 64x16 tile (one thread per 2x2 quad) and stages every window the tile needs in shared memory with
+// Here a CTA of 32x8 threads owns a 64x32 tile (a thread owns two vertically stacked 2x2 quads: what a thread pays per
+// tile and per covering image -- descriptors, window origins, border tests, barriers -- is paid once per eight pixels,
+// and the two quads share two of their three coarse rows) and stages every window the tile needs in shared memory with
 // asynchronous 16-byte copies (cp.async / LDGSTS, zero fill outside the source, the next image's windows in flight
-// while the current one is consumed): per covering image the 64x16 level-l pixels (level 0: packed RGBM; above: colour
-// words + weights) and the 34x10 window of level l+1 that holds the 3x3 pyrUp neighbourhoods of all quads, plus
-// the 34x10x3 window of the collapsed level C_{l+1}.  Elements outside a source arrive as zeros, which is exactly
+// while the current one is consumed): per covering image the 64x32 level-l pixels (level 0: packed RGBM; above: colour
+// words + weights) and the 34x18 window of level l+1 that holds the 3x3 pyrUp neighbourhoods of all quads, plus
+// the 34x18x3 window of the collapsed level C_{l+1}.  Elements outside a source arrive as zeros, which is exactly
 // "weight 0": no rect tests and no predicated taps in the consumers, whose shared-memory loads sit at compile-time
 // offsets.  The pyrUp is separable and neighbouring quads share two of their three coarse columns: every thread
-// computes the vertical column sums of ONE coarse column into shared memory and reads its three columns back (3 + 3
-// shared loads instead of 9 global ones per image, 9 + 6 instead of 27 for C_{l+1}).  The blend division, the
+// computes the vertical column sums of ONE coarse column for its two quad rows (four coarse rows read and split for two
+// rows of sums) into shared memory and reads its three columns back (per quad 2 + 3 shared loads instead of 9 global
+// ones per image, 6 + 6 instead of 27 for C_{l+1}).  The blend division, the
 // collapse add and |.| / min run on two 16-bit lanes per word (VIADD.16x2, VIMNMX.S16x2) with exact integer forms
 // for the weight sums 0, 1 and 2 that make up almost all of a panorama.
 //
@@ -41,7 +44,8 @@ namespace sb {
 
 namespace {
 
-constexpr int TW = SB_TILE_W, TH = SB_TILE_H, QX = TW / 2, QY = TH / 2;  // 64 x 16 pixels, 32 x 8 quads
+constexpr int TW = SB_TILE_W, TH = SB_TILE_H, QX = TW / 2, QY = TH / 2;  // 64 x 32 pixels, 32 x 16 quads
+constexpr int QT = 2, BY = QY / QT;  // quads per thread (rows QT ty .. QT ty + QT - 1 of the quad grid); the block is QX x BY threads
 constexpr int UPW = SB_TILE_UPW, UPH = SB_TILE_UPH;
 #define SB_WEIGHT_EPS 1e-5f
 
@@ -132,20 +136,27 @@ __device__ __forceinline__ void fix_borders(T (*t)[STRIDE], int bx, int by, int 
     __syncthreads();
 }
 
-// vertical column sums of coarse column `col` for the quads of row `row`: each colour word is split into the lanes
-// r | b << 16 and g (two 16-bit lanes per word; the largest value, 8 * 255, leaves room for the horizontal pass:
-// 8 * 2040 + 32 < 2^15)
+// vertical column sums of coarse column `col` for the quads of rows `row` .. `row + QT - 1`, which share all but one of
+// their coarse rows: each colour word is split into the lanes r | b << 16 and g (two 16-bit lanes per word; the largest
+// value, 8 * 255, leaves room for the horizontal pass: 8 * 2040 + 32 < 2^15)
 __device__ __forceinline__ void colsum_lanes(const uint32_t (*up)[UPS], uint4 (*cs)[UPW], int col, int row)  // col: logical column
 {
-    const unsigned a0 = up[row][col], a1 = up[row + 1][col], a2 = up[row + 2][col];
-    const unsigned M = 0x00ff00ffu;
-    const unsigned g0 = __byte_perm(a0, 0u, 0x4441), g1 = __byte_perm(a1, 0u, 0x4441), g2 = __byte_perm(a2, 0u, 0x4441);
-    uint4 v;
-    v.x = (a0 & M) + (a2 & M) + 6u * (a1 & M);  // even output row: 1 6 1
-    v.y = (a1 & M) + (a2 & M);                  // odd output row: 4 4 (the factor lives in the final shift)
-    v.z = g0 + g2 + 6u * g1;
-    v.w = g1 + g2;
-    cs[row][col] = v;
+    unsigned rb[QT + 2], g[QT + 2];
+#pragma unroll
+    for (int i = 0; i < QT + 2; ++i) {
+        const unsigned a = up[row + i][col];
+        rb[i] = a & 0x00ff00ffu;
+        g[i] = __byte_perm(a, 0u, 0x4441);
+    }
+#pragma unroll
+    for (int qy = 0; qy < QT; ++qy) {
+        uint4 v;
+        v.x = rb[qy] + rb[qy + 2] + 6u * rb[qy + 1];  // even output row: 1 6 1
+        v.y = rb[qy + 1] + rb[qy + 2];                // odd output row: 4 4 (the factor lives in the final shift)
+        v.z = g[qy] + g[qy + 2] + 6u * g[qy + 1];
+        v.w = g[qy + 1] + g[qy + 2];
+        cs[row + qy][col] = v;
+    }
 }
 
 __device__ __forceinline__ int lane_lo(unsigned v) { return (int)(short)(v & 0xffffu); }
@@ -173,10 +184,10 @@ __device__ __forceinline__ unsigned norm_two2(unsigned a)
     return __vadd2((xb >> 1) & 0x7fff7fffu, 0xfe00fe00u);                                   // - 512 per lane
 }
 
-// resident CTAs per SM: level 0 (24 KB of shared memory) 6; level 1 (33 KB with one colour word per pixel) 5 -- 48
-// registers, no spills (6 would spill)
+// resident CTAs per SM (2 x 256 quads each): level 0 (45 KB of shared memory) 4 at 64 registers; level 1 (62 KB) 3 at
+// 80 registers -- no spills
 template <int LV, bool SLABS>
-__global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 5) k_collapse_tile(const __grid_constant__ CollapseArgs A)
+__global__ void __launch_bounds__(QX *BY, LV == 0 ? 4 : 3) k_collapse_tile(const __grid_constant__ CollapseArgs A)
 {
     grid_dependency_sync();
 #ifndef SB_EMU
@@ -187,17 +198,22 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 5) k_collapse_tile(const
     Smem<LV> &S = *reinterpret_cast<Smem<LV> *>(smem_raw);
     const TileDesc *__restrict__ tile = A.tile;
     const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * QX + tx;
+    const int qr0 = QT * ty;  // the thread's first quad row
     const int tile_x = (A.rx0 & ~(TW - 1)) + blockIdx.x * TW, tile_y = A.ry0 + blockIdx.y * TH;  // staged rows start at 16-byte boundaries
 
-    // the collapsed level l+1 around the tile (3 planes x 10 rows x 6 chunks): in flight while the item list is built.
-    // Warp ty stages plane-rows 4 ty .. 4 ty + 3, eight lanes per row, six of them with a chunk.
+    // the collapsed level l+1 around the tile (3 planes x 18 rows x 6 chunks): in flight while the item list is built.
+    // Eight lanes per plane-row, six of them with a chunk; the block covers 32 plane-rows per pass.
     {
-        const int pr = 4 * ty + (tx >> 3), ch = tx & 7;
-        if (pr < 3 * UPH && ch < C1S / 8) {
-            const int plane = pr >= 2 * UPH ? 2 : (pr >= UPH ? 1 : 0), row = pr - UPH * plane;
-            const int xb = 2 * ((tile_x >> 1) - 1 - C1O) + 16 * ch;  // origin 32 k - 8 elements: a 16-byte boundary of an int16 row
-            stage_chunk(&S.c1[plane][row][8 * ch], A.up.c + (long long)plane * A.up.plane, 2u * (unsigned)A.up.pitch, (tile_y >> 1) - 1 + row,
-                        A.up.h_px, xb, (2 * A.up.w_px + 15) & ~15);
+        const int ch = tx & 7;
+#pragma unroll
+        for (int pr0 = 0; pr0 < 3 * UPH; pr0 += 4 * BY) {
+            const int pr = pr0 + 4 * ty + (tx >> 3);
+            if (pr < 3 * UPH && ch < C1S / 8) {
+                const int plane = pr >= 2 * UPH ? 2 : (pr >= UPH ? 1 : 0), row = pr - UPH * plane;
+                const int xb = 2 * ((tile_x >> 1) - 1 - C1O) + 16 * ch;  // origin 32 k - 8 elements: a 16-byte boundary of an int16 row
+                stage_chunk(&S.c1[plane][row][8 * ch], A.up.c + (long long)plane * A.up.plane, 2u * (unsigned)A.up.pitch, (tile_y >> 1) - 1 + row,
+                            A.up.h_px, xb, (2 * A.up.w_px + 15) & ~15);
+            }
         }
         cp_async_commit();
     }
@@ -221,8 +237,8 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 5) k_collapse_tile(const
     const int n_cover = S.list_n;
 
     // all threads: the asynchronous copies of item k's windows into buffer k & 1 (one commit group per item).  Warp ty
-    // stages rows 2 ty and 2 ty + 1 of the level-l windows and row ty (warps 0, 1 also rows 8, 9) of the coarse window,
-    // lane = chunk: no divisions, one address per thread and window.
+    // stages rows 4 ty .. 4 ty + 3 of the level-l windows and rows ty, ty + 8 (warps 0, 1 also ty + 16) of the coarse
+    // window, lane = chunk: no divisions, one address per thread and window.
     auto stage_item = [&](int k) {
         const int idx = S.list[k];
         const TileDesc &d = tile[idx];
@@ -234,41 +250,50 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 5) k_collapse_tile(const
         const int4 r = __ldg(reinterpret_cast<const int4 *>(&d.x0));   // x0, y0, w, h
         const int4 o = __ldg(reinterpret_cast<const int4 *>(&d.ox));   // ox, oy, uw, uh
         ItemBuf<LV> &B = S.item[k & 1];
-        if constexpr (LV == 0) {
-            if (tx < RGS / 4) {
+        if (tx < RGS / 4) {
+            const int rb = (4 * r.z + 15) & ~15;
+            if constexpr (LV == 0) {
                 const int xb = 4 * ((tile_x - r.x) & ~3) + 16 * tx;  // from the 16-byte boundary at or left of the tile
-                const int row = tile_y - r.y + 2 * ty;
+                const int row = tile_y - r.y + 2 * qr0;
                 const unsigned pb = 4u * (unsigned)cd.rgbm_pitch;
-                const int rb = (4 * r.z + 15) & ~15;
-                stage_chunk(&B.own[2 * ty][4 * tx], cd.rgbm, pb, row, r.w, xb, rb);
-                stage_chunk(&B.own[2 * ty + 1][4 * tx], cd.rgbm, pb, row + 1, r.w, xb, rb);
-            }
-        } else {
-            const int X = tile_x - o.x, row = tile_y - o.y + 2 * ty;  // X even (rect origins below the top level are even)
-            if (tx < RGS / 4) {  // colours and weights: same element size, same chunks
+#pragma unroll
+                for (int i = 0; i < 2 * QT; ++i) stage_chunk(&B.own[2 * qr0 + i][4 * tx], cd.rgbm, pb, row + i, r.w, xb, rb);
+            } else {  // colours and weights: same element size, same chunks
+                const int X = tile_x - o.x, row = tile_y - o.y + 2 * qr0;  // X even (rect origins below the top level are even)
                 const unsigned pb = 4u * (unsigned)cd.pitch;
-                const int xb = 4 * (X & ~3) + 16 * tx, rb = (4 * r.z + 15) & ~15;
-                stage_chunk(&B.own[2 * ty][4 * tx], cd.q, pb, row, r.w, xb, rb);
-                stage_chunk(&B.own[2 * ty + 1][4 * tx], cd.q, pb, row + 1, r.w, xb, rb);
-                stage_chunk(&B.w[2 * ty][4 * tx], cd.w, pb, row, r.w, xb, rb);
-                stage_chunk(&B.w[2 * ty + 1][4 * tx], cd.w, pb, row + 1, r.w, xb, rb);
+                const int xb = 4 * (X & ~3) + 16 * tx;
+#pragma unroll
+                for (int i = 0; i < 2 * QT; ++i) {
+                    stage_chunk(&B.own[2 * qr0 + i][4 * tx], cd.q, pb, row + i, r.w, xb, rb);
+                    stage_chunk(&B.w[2 * qr0 + i][4 * tx], cd.w, pb, row + i, r.w, xb, rb);
+                }
             }
         }
         if (tx < UPS / 4) {
             const int bx = (((tile_x - o.x) >> 1) - 1) & ~3, by = ((tile_y - o.y) >> 1) - 1;  // the multiple of 4 at or left of the origin
             const unsigned pb = 4u * (unsigned)cd.upitch;
             const int xb = 4 * bx + 16 * tx, rb = (4 * o.z + 15) & ~15;
-            stage_chunk(&B.up[ty][4 * tx], cd.uq, pb, by + ty, o.w, xb, rb);
-            if (ty < UPH - QY) stage_chunk(&B.up[QY + ty][4 * tx], cd.uq, pb, by + QY + ty, o.w, xb, rb);
+#pragma unroll
+            for (int row = 0; row < UPH; row += BY)
+                if (row + BY <= UPH || ty < UPH - row) stage_chunk(&B.up[row + ty][4 * tx], cd.uq, pb, by + row + ty, o.w, xb, rb);
         }
         cp_async_commit();
     };
     if (n_cover > 0) stage_item(0);
 
-    // accumulators of the quad (index dy * 2 + dx): red | blue << 16 as two wrap-around lanes, green, weight sum
-    unsigned acc_rb[4] = {0u, 0u, 0u, 0u};
-    int acc_g[4] = {0, 0, 0, 0};
-    float wsum[4] = {0.f, 0.f, 0.f, 0.f};
+    // accumulators of the thread's quads (index [quad][dy * 2 + dx]): red | blue << 16 as two wrap-around lanes, green,
+    // weight sum
+    unsigned acc_rb[QT][4];
+    int acc_g[QT][4];
+    float wsum[QT][4];
+#pragma unroll
+    for (int qy = 0; qy < QT; ++qy)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            acc_rb[qy][q] = 0u;
+            acc_g[qy][q] = 0;
+            wsum[qy][q] = 0.f;
+        }
 
     for (int k = 0; k < n_cover; ++k) {
         // item k+1 goes into the other buffer, whose last reader passed the second barrier of iteration k-1
@@ -287,17 +312,21 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 5) k_collapse_tile(const
                 // partial sums of another rank over (part of) this tile: int16 wrap-around adds, the float weight sum in
                 // item order (= rank order); rect origins and sizes are even: a quad is in or out as a whole
                 const int4 r = __ldg(reinterpret_cast<const int4 *>(&cd.ox));  // ox, oy, w_l, h_l
-                const int X = tile_x + 2 * tx - r.x, Y = tile_y + 2 * ty - r.y;
-                if ((unsigned)X < (unsigned)r.z && (unsigned)Y < (unsigned)r.w) {
-                    const int pitch = __ldg(&cd.pitch), plane = __ldg(&cd.plane);
-                    const int16_t *g = cd.g;
-                    const float *w = cd.w;
+                const int X = tile_x + 2 * tx - r.x;
+                const int pitch = __ldg(&cd.pitch), plane = __ldg(&cd.plane);
+                const int16_t *g = cd.g;
+                const float *w = cd.w;
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const int o = (Y + (q >> 1)) * pitch + X + (q & 1);
-                        acc_rb[q] = __vadd2(acc_rb[q], lanes(g[o], g[2 * plane + o]));
-                        acc_g[q] += g[plane + o];
-                        wsum[q] = fadd(wsum[q], w[o]);
+                for (int qy = 0; qy < QT; ++qy) {
+                    const int Y = tile_y + 2 * (qr0 + qy) - r.y;
+                    if ((unsigned)X < (unsigned)r.z && (unsigned)Y < (unsigned)r.w) {
+#pragma unroll
+                        for (int q = 0; q < 4; ++q) {
+                            const int o = (Y + (q >> 1)) * pitch + X + (q & 1);
+                            acc_rb[qy][q] = __vadd2(acc_rb[qy][q], lanes(g[o], g[2 * plane + o]));
+                            acc_g[qy][q] += g[plane + o];
+                            wsum[qy][q] = fadd(wsum[qy][q], w[o]);
+                        }
                     }
                 }
                 continue;  // (tile-uniform: no thread waits at the second barrier of this iteration)
@@ -311,73 +340,91 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 5) k_collapse_tile(const
         uint4(*cs)[UPW] = S.cs[k & 1];
         {
             const uint32_t(*ups)[UPS] = reinterpret_cast<const uint32_t(*)[UPS]>(&B.up[0][su]);
-            colsum_lanes(ups, cs, tx, ty);
-            if (tid < 2 * QY) colsum_lanes(ups, cs, QX + (tid & 1), tid >> 1);  // the two columns right of the last quad
+            colsum_lanes(ups, cs, tx, qr0);
+            if (tid < 2 * BY) colsum_lanes(ups, cs, QX + (tid & 1), QT * (tid >> 1));  // the two columns right of the last quad
         }
 
-        // the quad's own pixels: g_rb = r | b << 16, g_g = green, wt = weight
-        unsigned g_rb[4], g_g[4];
-        float wt[4];
-        bool nothing, unit;
+        // the quads' own pixels, read before the barrier and unpacked after it (level 0: RGBM words; above: colour
+        // words and weights)
+        unsigned p[QT][4];
+        float wt[QT][4];
         if constexpr (LV == 0) {
             const int sx = ((tile_x - __ldg(&d.x0)) & 3) + 2 * tx;  // the staged window starts at a multiple of 4 pixels
-            const unsigned p[4] = {B.own[2 * ty][sx], B.own[2 * ty][sx + 1], B.own[2 * ty + 1][sx], B.own[2 * ty + 1][sx + 1]};
-            nothing = ((p[0] | p[1] | p[2] | p[3]) >> 24) == 0u;           // all four weights are exactly 0
-            unit = ((p[0] & p[1] & p[2] & p[3]) >> 24) == 255u;             // all four weights are exactly 1
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                g_rb[q] = p[q] & 0x00ff00ffu;
-                g_g[q] = (p[q] >> 8) & 255u;
-                wt[q] = unit ? 1.f : fmul((float)(p[q] >> 24), SB_INV255);  // 255 * fl(1/255) == 1 exactly
-            }
+            for (int qy = 0; qy < QT; ++qy)
+#pragma unroll
+                for (int q = 0; q < 4; ++q) p[qy][q] = B.own[2 * (qr0 + qy) + (q >> 1)][sx + (q & 1)];
         } else {
             const int sw = ((tile_x - o.x) & 3) + 2 * tx;  // the staged windows start at a multiple of 4 columns
-            const float2 w0 = *reinterpret_cast<const float2 *>(&B.w[2 * ty][sw]);
-            const float2 w1 = *reinterpret_cast<const float2 *>(&B.w[2 * ty + 1][sw]);
-            const uint2 a = *reinterpret_cast<const uint2 *>(&B.own[2 * ty][sw]);
-            const uint2 b = *reinterpret_cast<const uint2 *>(&B.own[2 * ty + 1][sw]);
-            wt[0] = w0.x; wt[1] = w0.y; wt[2] = w1.x; wt[3] = w1.y;
-            const unsigned p[4] = {a.x, a.y, b.x, b.y};
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                g_rb[q] = p[q] & 0x00ff00ffu;
-                g_g[q] = __byte_perm(p[q], 0u, 0x4441);
-            }
-            nothing = wt[0] == 0.f && wt[1] == 0.f && wt[2] == 0.f && wt[3] == 0.f;
-            unit = wt[0] == 1.f && wt[1] == 1.f && wt[2] == 1.f && wt[3] == 1.f;
+            for (int qy = 0; qy < QT; ++qy)
+#pragma unroll
+                for (int dy = 0; dy < 2; ++dy) {
+                    const float2 w2 = *reinterpret_cast<const float2 *>(&B.w[2 * (qr0 + qy) + dy][sw]);
+                    const uint2 a = *reinterpret_cast<const uint2 *>(&B.own[2 * (qr0 + qy) + dy][sw]);
+                    wt[qy][2 * dy] = w2.x; wt[qy][2 * dy + 1] = w2.y;
+                    p[qy][2 * dy] = a.x; p[qy][2 * dy + 1] = a.y;
+                }
         }
         __syncthreads();        // the column sums of this image are complete
-        if (nothing) continue;  // (short)trunc(L * 0) == 0 and wsum + 0 == wsum: contributes exactly nothing
 
-        // pyrUp of the image's level l+1 at the four pixels: horizontal pass over the three column sums
-        const uint4 c0 = cs[ty][tx], c1 = cs[ty][tx + 1], c2 = cs[ty][tx + 2];
-        const unsigned M = 0x00ff00ffu;
-        unsigned u_rb[4], u_g[4];
-        u_rb[0] = ((c0.x + c2.x + 6u * c1.x + 0x00200020u) >> 6) & M;
-        u_rb[1] = ((c1.x + c2.x + 0x00080008u) >> 4) & M;
-        u_rb[2] = ((c0.y + c2.y + 6u * c1.y + 0x00080008u) >> 4) & M;
-        u_rb[3] = ((c1.y + c2.y + 0x00020002u) >> 2) & M;
-        u_g[0] = (c0.z + c2.z + 6u * c1.z + 32u) >> 6;
-        u_g[1] = (c1.z + c2.z + 8u) >> 4;
-        u_g[2] = (c0.w + c2.w + 6u * c1.w + 8u) >> 4;
-        u_g[3] = (c1.w + c2.w + 2u) >> 2;
-        if (unit) {  // (short)trunc(L * 1.0f) == L
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                acc_rb[q] = __vadd2(acc_rb[q], __vsub2(g_rb[q], u_rb[q]));
-                acc_g[q] += (int)g_g[q] - (int)u_g[q];
-                wsum[q] = fadd(wsum[q], 1.f);
+        for (int qy = 0; qy < QT; ++qy) {
+            // g_rb = r | b << 16, g_g = green, w = weight
+            unsigned g_rb[4], g_g[4];
+            float w[4];
+            bool nothing, unit;
+            if constexpr (LV == 0) {
+                nothing = ((p[qy][0] | p[qy][1] | p[qy][2] | p[qy][3]) >> 24) == 0u;  // all four weights are exactly 0
+                unit = ((p[qy][0] & p[qy][1] & p[qy][2] & p[qy][3]) >> 24) == 255u;    // all four weights are exactly 1
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    g_rb[q] = p[qy][q] & 0x00ff00ffu;
+                    g_g[q] = (p[qy][q] >> 8) & 255u;
+                    w[q] = unit ? 1.f : fmul((float)(p[qy][q] >> 24), SB_INV255);  // 255 * fl(1/255) == 1 exactly
+                }
+            } else {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    w[q] = wt[qy][q];
+                    g_rb[q] = p[qy][q] & 0x00ff00ffu;
+                    g_g[q] = __byte_perm(p[qy][q], 0u, 0x4441);
+                }
+                nothing = w[0] == 0.f && w[1] == 0.f && w[2] == 0.f && w[3] == 0.f;
+                unit = w[0] == 1.f && w[1] == 1.f && w[2] == 1.f && w[3] == 1.f;
             }
-        } else {
+            if (nothing) continue;  // (short)trunc(L * 0) == 0 and wsum + 0 == wsum: contributes exactly nothing
+
+            // pyrUp of the image's level l+1 at the four pixels: horizontal pass over the three column sums
+            const uint4 c0 = cs[qr0 + qy][tx], c1 = cs[qr0 + qy][tx + 1], c2 = cs[qr0 + qy][tx + 2];
+            const unsigned M = 0x00ff00ffu;
+            unsigned u_rb[4], u_g[4];
+            u_rb[0] = ((c0.x + c2.x + 6u * c1.x + 0x00200020u) >> 6) & M;
+            u_rb[1] = ((c1.x + c2.x + 0x00080008u) >> 4) & M;
+            u_rb[2] = ((c0.y + c2.y + 6u * c1.y + 0x00080008u) >> 4) & M;
+            u_rb[3] = ((c1.y + c2.y + 0x00020002u) >> 2) & M;
+            u_g[0] = (c0.z + c2.z + 6u * c1.z + 32u) >> 6;
+            u_g[1] = (c1.z + c2.z + 8u) >> 4;
+            u_g[2] = (c0.w + c2.w + 6u * c1.w + 8u) >> 4;
+            u_g[3] = (c1.w + c2.w + 2u) >> 2;
+            if (unit) {  // (short)trunc(L * 1.0f) == L
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const unsigned lap_rb = __vsub2(g_rb[q], u_rb[q]);
-                const int lap_g = (int)g_g[q] - (int)u_g[q];
-                const int tr = trunc16(fmul((float)lane_lo(lap_rb), wt[q]));
-                const int tb = trunc16(fmul((float)lane_hi(lap_rb), wt[q]));
-                acc_rb[q] = __vadd2(acc_rb[q], lanes(tr, tb));
-                acc_g[q] += trunc16(fmul((float)lap_g, wt[q]));
-                wsum[q] = fadd(wsum[q], wt[q]);
+                for (int q = 0; q < 4; ++q) {
+                    acc_rb[qy][q] = __vadd2(acc_rb[qy][q], __vsub2(g_rb[q], u_rb[q]));
+                    acc_g[qy][q] += (int)g_g[q] - (int)u_g[q];
+                    wsum[qy][q] = fadd(wsum[qy][q], 1.f);
+                }
+            } else {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const unsigned lap_rb = __vsub2(g_rb[q], u_rb[q]);
+                    const int lap_g = (int)g_g[q] - (int)u_g[q];
+                    const int tr = trunc16(fmul((float)lane_lo(lap_rb), w[q]));
+                    const int tb = trunc16(fmul((float)lane_hi(lap_rb), w[q]));
+                    acc_rb[qy][q] = __vadd2(acc_rb[qy][q], lanes(tr, tb));
+                    acc_g[qy][q] += trunc16(fmul((float)lap_g, w[q]));
+                    wsum[qy][q] = fadd(wsum[qy][q], w[q]);
+                }
             }
         }
     }
@@ -398,136 +445,150 @@ __global__ void __launch_bounds__(QX *QY, LV == 0 ? 6 : 5) k_collapse_tile(const
     __syncthreads();  // nobody reads the images' column sums any more: the buffers now take those of C_{l+1}
     int4(*csa)[UPW] = reinterpret_cast<int4(*)[UPW]>(S.cs[0]);   // e_r, e_g, e_b, o_r
     int2(*csb)[UPW] = reinterpret_cast<int2(*)[UPW]>(S.cs[1]);   // o_g, o_b
-    auto colsum_c = [&](int col, int row) {
-        int e[3], od[3];
+    auto colsum_c = [&](int col, int row) {  // quad rows row .. row + QT - 1
+        int e[QT][3], od[QT][3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-            const int a0 = S.c1[c][row][col + C1O], a1 = S.c1[c][row + 1][col + C1O], a2 = S.c1[c][row + 2][col + C1O];
-            e[c] = a0 + a2 + 6 * a1;
-            od[c] = a1 + a2;
+            int a[QT + 2];
+#pragma unroll
+            for (int i = 0; i < QT + 2; ++i) a[i] = S.c1[c][row + i][col + C1O];
+#pragma unroll
+            for (int qy = 0; qy < QT; ++qy) {
+                e[qy][c] = a[qy] + a[qy + 2] + 6 * a[qy + 1];
+                od[qy][c] = a[qy + 1] + a[qy + 2];
+            }
         }
-        csa[row][col] = make_int4(e[0], e[1], e[2], od[0]);
-        csb[row][col] = make_int2(od[1], od[2]);
+#pragma unroll
+        for (int qy = 0; qy < QT; ++qy) {
+            csa[row + qy][col] = make_int4(e[qy][0], e[qy][1], e[qy][2], od[qy][0]);
+            csb[row + qy][col] = make_int2(od[qy][1], od[qy][2]);
+        }
     };
-    colsum_c(tx, ty);
-    if (tid < 2 * QY) colsum_c(QX + (tid & 1), tid >> 1);
+    colsum_c(tx, qr0);
+    if (tid < 2 * BY) colsum_c(QX + (tid & 1), QT * (tid >> 1));
     __syncthreads();
-    int u[3][4];  // [channel][pixel of the quad]
-    {
-        const int4 a0 = csa[ty][tx], a1 = csa[ty][tx + 1], a2 = csa[ty][tx + 2];
-        const int2 b0 = csb[ty][tx], b1 = csb[ty][tx + 1], b2 = csb[ty][tx + 2];
-        const int e0[3] = {a0.x, a0.y, a0.z}, e1[3] = {a1.x, a1.y, a1.z}, e2[3] = {a2.x, a2.y, a2.z};
-        const int o0[3] = {a0.w, b0.x, b0.y}, o1[3] = {a1.w, b1.x, b1.y}, o2[3] = {a2.w, b2.x, b2.y};
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            u[c][0] = (e0[c] + e2[c] + 6 * e1[c] + 32) >> 6;
-            u[c][1] = (e1[c] + e2[c] + 8) >> 4;
-            u[c][2] = (o0[c] + o2[c] + 6 * o1[c] + 8) >> 4;
-            u[c][3] = (o1[c] + o2[c] + 2) >> 2;
-        }
-    }
 
-    const int x = tile_x + 2 * tx, y = tile_y + 2 * ty;  // top-left pixel of the quad
-    if (x < A.rx0 || x >= A.rx0 + A.rw || y >= A.ry0 + A.rh) return;  // (after the last barrier)
-
-    // ---- blend step on lanes: words [row][0] = pixel 0 (r | b << 16), [row][1] = pixel 1, [row][2] = green of both ------
-    unsigned N[2][3];
-    const bool unit = (wsum[0] == 1.f || wsum[0] == 0.f) && (wsum[1] == 1.f || wsum[1] == 0.f) && (wsum[2] == 1.f || wsum[2] == 0.f) &&
-                      (wsum[3] == 1.f || wsum[3] == 0.f);
-    const bool two = wsum[0] == 2.f && wsum[1] == 2.f && wsum[2] == 2.f && wsum[3] == 2.f;
+    const int x = tile_x + 2 * tx;  // left pixel of the quads
+    if (x < A.rx0 || x >= A.rx0 + A.rw) return;  // (after the last barrier)
 #pragma unroll
-    for (int dy = 0; dy < 2; ++dy) {
-        N[dy][0] = acc_rb[2 * dy];
-        N[dy][1] = acc_rb[2 * dy + 1];
-        N[dy][2] = __byte_perm((unsigned)acc_g[2 * dy], (unsigned)acc_g[2 * dy + 1], 0x5410);
-    }
-    if (unit) {
+    for (int qy = 0; qy < QT; ++qy) {
+        const int y = tile_y + 2 * (qr0 + qy);  // top pixel of the quad
+        if (y >= A.ry0 + A.rh) return;
+        int u[3][4];  // [channel][pixel of the quad]
+        {
+            const int4 a0 = csa[qr0 + qy][tx], a1 = csa[qr0 + qy][tx + 1], a2 = csa[qr0 + qy][tx + 2];
+            const int2 b0 = csb[qr0 + qy][tx], b1 = csb[qr0 + qy][tx + 1], b2 = csb[qr0 + qy][tx + 2];
+            const int e0[3] = {a0.x, a0.y, a0.z}, e1[3] = {a1.x, a1.y, a1.z}, e2[3] = {a2.x, a2.y, a2.z};
+            const int o0[3] = {a0.w, b0.x, b0.y}, o1[3] = {a1.w, b1.x, b1.y}, o2[3] = {a2.w, b2.x, b2.y};
 #pragma unroll
-        for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-            for (int j = 0; j < 3; ++j) N[dy][j] = norm_unit2(N[dy][j]);
-    } else if (two) {
-#pragma unroll
-        for (int dy = 0; dy < 2; ++dy)
-#pragma unroll
-            for (int j = 0; j < 3; ++j) N[dy][j] = norm_two2(N[dy][j]);
-    } else {  // fractional weight sums: one refined reciprocal per pixel, an exact quotient per channel (sb_device.cuh)
-#pragma unroll
-        for (int dy = 0; dy < 2; ++dy) {
-            int n[2][3];
-#pragma unroll
-            for (int dx = 0; dx < 2; ++dx) {
-                const float den = fadd(wsum[2 * dy + dx], SB_WEIGHT_EPS);
-                const float rr = rcp_refined(den);
-                n[dx][0] = norm16(lane_lo(N[dy][dx]), den, rr);
-                n[dx][1] = norm16(dx ? lane_hi(N[dy][2]) : lane_lo(N[dy][2]), den, rr);
-                n[dx][2] = norm16(lane_hi(N[dy][dx]), den, rr);
-            }
-            N[dy][0] = lanes(n[0][0], n[0][2]);
-            N[dy][1] = lanes(n[1][0], n[1][2]);
-            N[dy][2] = lanes(n[0][1], n[1][1]);
-        }
-    }
-    // collapse add: |pyrUp| <= 256 (nb - l) and |n| <= 255 for byte-fed images, far inside int16: the lane-wise
-    // wrap-around add equals the reference's saturating add
-    unsigned V[2][3];
-#pragma unroll
-    for (int dy = 0; dy < 2; ++dy) {
-        V[dy][0] = __vadd2(N[dy][0], lanes(u[0][2 * dy], u[2][2 * dy]));
-        V[dy][1] = __vadd2(N[dy][1], lanes(u[0][2 * dy + 1], u[2][2 * dy + 1]));
-        V[dy][2] = __vadd2(N[dy][2], lanes(u[1][2 * dy], u[1][2 * dy + 1]));
-    }
-    if (LV == 1) {  // C_l: three int16 planes, two pixels per 4-byte store
-#pragma unroll
-        for (int dy = 0; dy < 2; ++dy) {
-            const int o = (y + dy) * A.cur.pitch + x;
-            *reinterpret_cast<unsigned *>(A.cur.c + o) = __byte_perm(V[dy][0], V[dy][1], 0x5410);
-            *reinterpret_cast<unsigned *>(A.cur.c + A.cur.plane + o) = V[dy][2];
-            *reinterpret_cast<unsigned *>(A.cur.c + 2 * A.cur.plane + o) = __byte_perm(V[dy][0], V[dy][1], 0x7632);
-        }
-        return;
-    }
-    // level 0: mask, zero outside it, |v| saturated to uint8 (convertScaleAbs), crop to the roi
-    const PanoOut &out = A.out;
-    const unsigned xo = (unsigned)(x - A.out_x0);
-    unsigned o_rgb = (unsigned)y * (unsigned)out.rgb_pitch + 3u * xo, o_m = (unsigned)y * (unsigned)out.mask_pitch + xo;
-    const bool both = x >= A.out_lo && x + 1 < A.out_hi;
-#pragma unroll
-    for (int dy = 0; dy < 2; ++dy) {
-        if (y + dy < out.h) {
-            const unsigned m0 = wsum[2 * dy] > SB_WEIGHT_EPS ? 0xffffffffu : 0u, m1 = wsum[2 * dy + 1] > SB_WEIGHT_EPS ? 0xffffffffu : 0u;
-            unsigned Bq[3];
-#pragma unroll
-            for (int j = 0; j < 3; ++j) Bq[j] = __vmins2(__viaddmax_s16x2(~V[dy][j], 0x00010001u, V[dy][j]), 0x00ff00ffu);  // min(max(-v, v), 255)
-            Bq[0] &= m0;
-            Bq[1] &= m1;
-            Bq[2] &= __byte_perm(m0, m1, 0x5410);
-            // bytes r0 g0 | b0 r1 | g1 b1
-            const unsigned h0 = __byte_perm(Bq[0], Bq[2], 0x0040), h1 = __byte_perm(Bq[0], Bq[1], 0x0042), h2 = __byte_perm(Bq[2], Bq[1], 0x0062);
-            const unsigned hm = __byte_perm(m0, m1, 0x0040);
-            if (both) {
-                unsigned short *p2 = reinterpret_cast<unsigned short *>(out.rgb + o_rgb);
-                p2[0] = (unsigned short)h0;
-                p2[1] = (unsigned short)h1;
-                p2[2] = (unsigned short)h2;
-                *reinterpret_cast<unsigned short *>(out.mask + o_m) = (unsigned short)hm;
-            } else {  // the roi's last (odd) column, or a column outside [out_lo, out_hi)
-                if (x >= A.out_lo && x < A.out_hi) {
-                    out.rgb[o_rgb] = (uint8_t)h0;
-                    out.rgb[o_rgb + 1] = (uint8_t)(h0 >> 8);
-                    out.rgb[o_rgb + 2] = (uint8_t)h1;
-                    out.mask[o_m] = (uint8_t)hm;
-                }
-                if (x + 1 >= A.out_lo && x + 1 < A.out_hi) {
-                    out.rgb[o_rgb + 3] = (uint8_t)(h1 >> 8);
-                    out.rgb[o_rgb + 4] = (uint8_t)h2;
-                    out.rgb[o_rgb + 5] = (uint8_t)(h2 >> 8);
-                    out.mask[o_m + 1] = (uint8_t)(hm >> 8);
-                }
+            for (int c = 0; c < 3; ++c) {
+                u[c][0] = (e0[c] + e2[c] + 6 * e1[c] + 32) >> 6;
+                u[c][1] = (e1[c] + e2[c] + 8) >> 4;
+                u[c][2] = (o0[c] + o2[c] + 6 * o1[c] + 8) >> 4;
+                u[c][3] = (o1[c] + o2[c] + 2) >> 2;
             }
         }
-        o_rgb += (unsigned)out.rgb_pitch;
-        o_m += (unsigned)out.mask_pitch;
+
+        // ---- blend step on lanes: words [row][0] = pixel 0 (r | b << 16), [row][1] = pixel 1, [row][2] = green of both --
+        const float(&ws)[4] = wsum[qy];
+        unsigned N[2][3];
+        const bool unit = (ws[0] == 1.f || ws[0] == 0.f) && (ws[1] == 1.f || ws[1] == 0.f) && (ws[2] == 1.f || ws[2] == 0.f) &&
+                          (ws[3] == 1.f || ws[3] == 0.f);
+        const bool two = ws[0] == 2.f && ws[1] == 2.f && ws[2] == 2.f && ws[3] == 2.f;
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy) {
+            N[dy][0] = acc_rb[qy][2 * dy];
+            N[dy][1] = acc_rb[qy][2 * dy + 1];
+            N[dy][2] = __byte_perm((unsigned)acc_g[qy][2 * dy], (unsigned)acc_g[qy][2 * dy + 1], 0x5410);
+        }
+        if (unit) {
+#pragma unroll
+            for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+                for (int j = 0; j < 3; ++j) N[dy][j] = norm_unit2(N[dy][j]);
+        } else if (two) {
+#pragma unroll
+            for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+                for (int j = 0; j < 3; ++j) N[dy][j] = norm_two2(N[dy][j]);
+        } else {  // fractional weight sums: one refined reciprocal per pixel, an exact quotient per channel (sb_device.cuh)
+#pragma unroll
+            for (int dy = 0; dy < 2; ++dy) {
+                int n[2][3];
+#pragma unroll
+                for (int dx = 0; dx < 2; ++dx) {
+                    const float den = fadd(ws[2 * dy + dx], SB_WEIGHT_EPS);
+                    const float rr = rcp_refined(den);
+                    n[dx][0] = norm16(lane_lo(N[dy][dx]), den, rr);
+                    n[dx][1] = norm16(dx ? lane_hi(N[dy][2]) : lane_lo(N[dy][2]), den, rr);
+                    n[dx][2] = norm16(lane_hi(N[dy][dx]), den, rr);
+                }
+                N[dy][0] = lanes(n[0][0], n[0][2]);
+                N[dy][1] = lanes(n[1][0], n[1][2]);
+                N[dy][2] = lanes(n[0][1], n[1][1]);
+            }
+        }
+        // collapse add: |pyrUp| <= 256 (nb - l) and |n| <= 255 for byte-fed images, far inside int16: the lane-wise
+        // wrap-around add equals the reference's saturating add
+        unsigned V[2][3];
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy) {
+            V[dy][0] = __vadd2(N[dy][0], lanes(u[0][2 * dy], u[2][2 * dy]));
+            V[dy][1] = __vadd2(N[dy][1], lanes(u[0][2 * dy + 1], u[2][2 * dy + 1]));
+            V[dy][2] = __vadd2(N[dy][2], lanes(u[1][2 * dy], u[1][2 * dy + 1]));
+        }
+        if constexpr (LV == 1) {  // C_l: three int16 planes, two pixels per 4-byte store
+#pragma unroll
+            for (int dy = 0; dy < 2; ++dy) {
+                const int o = (y + dy) * A.cur.pitch + x;
+                *reinterpret_cast<unsigned *>(A.cur.c + o) = __byte_perm(V[dy][0], V[dy][1], 0x5410);
+                *reinterpret_cast<unsigned *>(A.cur.c + A.cur.plane + o) = V[dy][2];
+                *reinterpret_cast<unsigned *>(A.cur.c + 2 * A.cur.plane + o) = __byte_perm(V[dy][0], V[dy][1], 0x7632);
+            }
+        } else {
+            // level 0: mask, zero outside it, |v| saturated to uint8 (convertScaleAbs), crop to the roi
+            const PanoOut &out = A.out;
+            const unsigned xo = (unsigned)(x - A.out_x0);
+            unsigned o_rgb = (unsigned)y * (unsigned)out.rgb_pitch + 3u * xo, o_m = (unsigned)y * (unsigned)out.mask_pitch + xo;
+            const bool both = x >= A.out_lo && x + 1 < A.out_hi;
+#pragma unroll
+            for (int dy = 0; dy < 2; ++dy) {
+                if (y + dy < out.h) {
+                    const unsigned m0 = ws[2 * dy] > SB_WEIGHT_EPS ? 0xffffffffu : 0u, m1 = ws[2 * dy + 1] > SB_WEIGHT_EPS ? 0xffffffffu : 0u;
+                    unsigned Bq[3];
+#pragma unroll
+                    for (int j = 0; j < 3; ++j) Bq[j] = __vmins2(__viaddmax_s16x2(~V[dy][j], 0x00010001u, V[dy][j]), 0x00ff00ffu);  // min(max(-v, v), 255)
+                    Bq[0] &= m0;
+                    Bq[1] &= m1;
+                    Bq[2] &= __byte_perm(m0, m1, 0x5410);
+                    // bytes r0 g0 | b0 r1 | g1 b1
+                    const unsigned h0 = __byte_perm(Bq[0], Bq[2], 0x0040), h1 = __byte_perm(Bq[0], Bq[1], 0x0042), h2 = __byte_perm(Bq[2], Bq[1], 0x0062);
+                    const unsigned hm = __byte_perm(m0, m1, 0x0040);
+                    if (both) {
+                        unsigned short *p2 = reinterpret_cast<unsigned short *>(out.rgb + o_rgb);
+                        p2[0] = (unsigned short)h0;
+                        p2[1] = (unsigned short)h1;
+                        p2[2] = (unsigned short)h2;
+                        *reinterpret_cast<unsigned short *>(out.mask + o_m) = (unsigned short)hm;
+                    } else {  // the roi's last (odd) column, or a column outside [out_lo, out_hi)
+                        if (x >= A.out_lo && x < A.out_hi) {
+                            out.rgb[o_rgb] = (uint8_t)h0;
+                            out.rgb[o_rgb + 1] = (uint8_t)(h0 >> 8);
+                            out.rgb[o_rgb + 2] = (uint8_t)h1;
+                            out.mask[o_m] = (uint8_t)hm;
+                        }
+                        if (x + 1 >= A.out_lo && x + 1 < A.out_hi) {
+                            out.rgb[o_rgb + 3] = (uint8_t)(h1 >> 8);
+                            out.rgb[o_rgb + 4] = (uint8_t)h2;
+                            out.rgb[o_rgb + 5] = (uint8_t)(h2 >> 8);
+                            out.mask[o_m + 1] = (uint8_t)(hm >> 8);
+                        }
+                    }
+                }
+                o_rgb += (unsigned)out.rgb_pitch;
+                o_m += (unsigned)out.mask_pitch;
+            }
+        }
     }
 }
 
@@ -575,7 +636,7 @@ int launch_collapse_tile(const CollapseArgs &A, int l, int nb, cudaStream_t s)
         attr_set = true;
     }
 #endif
-    dim3 block(QX, QY), grid(div_up(A.rx0 + A.rw - (A.rx0 & ~(TW - 1)), TW), div_up(A.rh, TH));
+    dim3 block(QX, BY), grid(div_up(A.rx0 + A.rw - (A.rx0 & ~(TW - 1)), TW), div_up(A.rh, TH));
 #ifdef SB_EMU
     if (getenv("SB_EMU_TRACE")) fprintf(stderr, "k_collapse_tile<%d, %d> %ux%u tiles, %d items\n", l, A.has_slabs, grid.x, grid.y, A.n);
 #endif

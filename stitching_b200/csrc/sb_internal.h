@@ -169,11 +169,11 @@ struct alignas(16) TileDesc {
     int x0, y0, w, h;           // level 0: the fed IMAGE inside its padded rect (weights are 0 outside); levels >= 1: the padded rect
     int ox, oy, uw, uh;         // padded rect origin at this level; size of the next coarser level (source of the pyrUp)
 };
-// window shapes of the tile kernels (one CTA = TILE_W x TILE_H pixels of a level, one thread per 2x2 quad)
+// window shapes of the tile kernels (one CTA = TILE_W x TILE_H pixels of a level, one thread per two stacked 2x2 quads)
 #define SB_TILE_W 64
-#define SB_TILE_H 16
+#define SB_TILE_H 32
 #define SB_TILE_UPW (SB_TILE_W / 2 + 2)   // 34: the 3x3 neighbourhoods of the tile's quads at the coarser level
-#define SB_TILE_UPH (SB_TILE_H / 2 + 2)   // 10
+#define SB_TILE_UPH (SB_TILE_H / 2 + 2)   // 18
 
 struct PanoLevel {
     int16_t *c;  // collapsed planar int16 x3 [3][h][pitch]
