@@ -24,14 +24,41 @@ using namespace sb;
 
 #define SB_PIPE_DEPTH 3  // buffer sets of the pipelined submit / wait path
 
+// One image of the rig.  Its buffers exist when this compositor warps it (listed in sb_compositor::warped: its own block,
+// on the timelapse canvas); the other images keep them null.
+struct Image {
+    int w = 0, h = 0;             // FINAL size: what is warped
+    int in_w = 0, in_h = 0;       // the frames upload / submit take: w x h unless resized on the device
+    int *taps = nullptr;          // resized on the device (sb_compositor_opts.in_w / in_h): [x taps | y taps] (resize_exact_taps)
+    bool words = false;           // the warp kernel reads the source as one word per pixel, else packed u8x3 (plan_sources)
+    Rect rect{};                  // fed rect (pano-absolute)
+    Rect part{};                  // timelapse: the fed rect on the canvas (P_i, pano-absolute; w = h = 0 when empty)
+    size_t paste_off = 0;         // timelapse: its block in Slot::paste
+    WarpJob job{};                // its warp job without sources (warp_jobs adds a slot's)
+    uint32_t *rgbm = nullptr;     // warped, packed; row pitch = width rounded up to 32 pixels (128-byte rows)
+    float *tab = nullptr;
+    float *maps = nullptr;        // projections that are not separable: xmap | ymap (built at plan time)
+    uint8_t *usermask = nullptr;  // blend mask (sb_compositor_set_mask / _set_seam_mask)
+    GainData gain;                // exposure gains (sb_compositor_set_gain)
+};
+
+static void image_free(Image &im, cudaStream_t s)
+{
+    for (void *p : {(void *)im.taps, (void *)im.rgbm, (void *)im.tab, (void *)im.maps, (void *)im.usermask}) dev_free(p, s);
+    gain_free(&im.gain, s);
+}
+
+// The sources of one image in one slot (null for an image this compositor does not warp)
+struct SlotImage {
+    uint8_t *frame = nullptr;  // the frame as uploaded: u8x3 at the input size
+    void *src = nullptr;       // what the warp reads in its place, written after every upload: the words (Image::words), or
+                               // the packed FINAL-size frame of a resized image; null for a packed image that is not resized
+};
+
 // One buffer set.  Slot 0 serves upload / run / download, the timing calls and the sharded step; the pipelined
 // submit / wait path deals its steps round-robin to all SB_PIPE_DEPTH slots.
 struct Slot {
-    std::vector<uint8_t *> src;    // u8x3 sources as uploaded (null: an image of another rank)
-    std::vector<uint32_t *> src4;  // the same, one word per pixel: what the warp kernel reads (repacked after every upload)
-    // An image resized on the device (sb_compositor_opts.in_w / in_h) has its camera-size frame in `src` and its FINAL-size
-    // source, written by k_resize_src, in `src4` when the warp kernel reads words, else in `fin` (packed u8x3).
-    std::vector<uint8_t *> fin;
+    std::vector<SlotImage> img;    // per image
     PanoOut out{};                 // device outputs
     // timelapse (sb_compositor_opts.timelapse): the pasted parts of the frames, one 16-byte aligned block per image with a
     // non-empty part; their k_timelapse_paste jobs; the n page-locked frames of the canvas this slot's steps end in
@@ -47,21 +74,10 @@ struct Slot {
 struct sb_compositor {
     int n = 0;
     cudaStream_t stream = nullptr;
-    std::vector<int> src_w, src_h;     // FINAL sizes: what is warped
-    std::vector<int> in_w, in_h;       // the frames upload / submit take: src_w / src_h unless resized on the device
-    std::vector<int *> taps_dev;       // resized images: [x taps | y taps] (resize_exact_taps), null for the others
-    std::vector<char> warp_src4;       // resized images: the warp kernel reads the word-per-pixel source
-    std::vector<ResizeJob> resize_jobs;  // scratch of prepare_sources
-    std::vector<Rect> rects;           // warped rects (pano-absolute)
+    std::vector<Image> img;            // per image
     std::vector<int> warped;           // the images this compositor warps, in launch order (set at creation)
-    std::vector<WarpJob> jobs;         // per image: its warp job without sources (warp_jobs adds a slot's)
+    std::vector<ResizeJob> resize_jobs;  // scratch of prepare_sources
     std::vector<WarpJob> step_jobs;    // scratch of warp_jobs
-    bool use_src4 = true;
-    std::vector<uint32_t *> rgbm_dev;  // warped, packed; row pitch = width rounded up to 32 pixels (128-byte rows)
-    std::vector<float *> tab_dev;
-    std::vector<float *> maps_dev;     // projections that are not separable: xmap | ymap of every image (built at plan time)
-    std::vector<uint8_t *> usermask_dev;
-    std::vector<GainData> gain;        // exposure gains per image (sb_compositor_set_gain)
     BlendPlan plan;
     Slot slots[SB_PIPE_DEPTH];
     int n_slots = 0;                   // slots with buffers: 1 from creation, all from the first submit on
@@ -85,8 +101,6 @@ struct sb_compositor {
     // timelapse mode: no blend plan; every step writes one frame of the canvas per image (cv.detail.Timelapser)
     int timelapse = 0;                 // 0, SB_TIMELAPSE_AS_IS or SB_TIMELAPSE_CROP
     Rect canvas{0, 0, 0, 0};           // resultRoi / resultRoiIntersection of the fed rects (pano-absolute)
-    std::vector<Rect> part;            // per image: its fed rect on the canvas (P_i, pano-absolute; w = h = 0 when empty)
-    std::vector<size_t> paste_off;     // per image: its block in Slot::paste
     size_t paste_bytes = 0;
     long long paste_max = 0;           // largest 3 * |P_i|
     double paste_model = 0;            // model bytes of k_timelapse_paste
@@ -96,21 +110,16 @@ struct sb_compositor {
 static int slot_alloc(sb_compositor *c, Slot &sl)
 {
     cudaStream_t s = c->stream;
-    sl.src.assign(c->n, nullptr);
-    sl.src4.assign(c->n, nullptr);
-    sl.fin.assign(c->n, nullptr);
+    sl.img.assign(c->n, SlotImage{});
     for (int i : c->warped) {
-        const long long px = (long long)c->src_w[i] * c->src_h[i];
-        if (c->taps_dev[i]) {
-            SB_TRY(dev_alloc((void **)&sl.src[i], (size_t)c->in_w[i] * c->in_h[i] * 3 + SB_SRC_PAD, s));
-            if (c->warp_src4[i])
-                SB_TRY(dev_alloc((void **)&sl.src4[i], ((size_t)px + 4) * sizeof(uint32_t), s));
-            else
-                SB_TRY(dev_alloc((void **)&sl.fin[i], (size_t)px * 3 + SB_SRC_PAD, s));
-            continue;
-        }
-        SB_TRY(dev_alloc((void **)&sl.src[i], (size_t)px * 3 + SB_SRC_PAD, s));
-        if (c->use_src4 && px < (1ll << 31)) SB_TRY(dev_alloc((void **)&sl.src4[i], ((size_t)px + 4) * sizeof(uint32_t), s));
+        const Image &im = c->img[i];
+        SlotImage &si = sl.img[i];
+        const size_t px = (size_t)im.w * im.h;
+        SB_TRY(dev_alloc((void **)&si.frame, (size_t)im.in_w * im.in_h * 3 + SB_SRC_PAD, s));
+        if (im.words)
+            SB_TRY(dev_alloc(&si.src, (px + 4) * sizeof(uint32_t), s));
+        else if (im.taps)
+            SB_TRY(dev_alloc(&si.src, px * 3 + SB_SRC_PAD, s));
     }
     SB_CUDA(cudaEventCreateWithFlags(&sl.e_h2d, cudaEventDisableTiming));
     SB_CUDA(cudaEventCreateWithFlags(&sl.e_comp, cudaEventDisableTiming));
@@ -119,8 +128,10 @@ static int slot_alloc(sb_compositor *c, Slot &sl)
         if (c->warped.empty()) return SB_OK;
         SB_TRY(dev_alloc((void **)&sl.paste, c->paste_bytes, s));
         std::vector<PasteJob> pj;
-        for (int i : c->warped)
-            pj.push_back(PasteJob{c->rgbm_dev[i], sl.paste + c->paste_off[i], rgbm_pitch_of(c->part[i].w), c->part[i].w, c->part[i].h});
+        for (int i : c->warped) {
+            const Image &im = c->img[i];
+            pj.push_back(PasteJob{im.rgbm, sl.paste + im.paste_off, rgbm_pitch_of(im.part.w), im.part.w, im.part.h});
+        }
         SB_TRY(dev_alloc((void **)&sl.paste_jobs, pj.size() * sizeof(PasteJob), s));
         SB_CUDA(cudaMemcpyAsync(sl.paste_jobs, pj.data(), pj.size() * sizeof(PasteJob), cudaMemcpyHostToDevice, s));
         SB_CUDA(cudaStreamSynchronize(s));  // pj goes out of scope
@@ -138,9 +149,10 @@ static int slot_alloc(sb_compositor *c, Slot &sl)
 
 static void slot_free(Slot &sl, cudaStream_t s)
 {
-    for (auto p : sl.src) dev_free(p, s);
-    for (auto p : sl.src4) dev_free(p, s);
-    for (auto p : sl.fin) dev_free(p, s);
+    for (SlotImage &si : sl.img) {
+        dev_free(si.frame, s);
+        dev_free(si.src, s);
+    }
     dev_free(sl.out.rgb, s);
     dev_free(sl.out.mask, s);
     dev_free(sl.paste, s);
@@ -160,12 +172,7 @@ static void compositor_free(sb_compositor *c)
     for (cudaStream_t q : {c->stream, c->h2d, c->d2h, c->comm_stream})  // nothing queued may still use what is freed
         if (q) (void)cudaStreamSynchronize(q);
     for (Slot &sl : c->slots) slot_free(sl, s);
-    for (auto p : c->rgbm_dev) dev_free(p, s);
-    for (auto p : c->tab_dev) dev_free(p, s);
-    for (auto p : c->maps_dev) dev_free(p, s);
-    for (auto p : c->usermask_dev) dev_free(p, s);
-    for (auto p : c->taps_dev) dev_free(p, s);
-    for (auto &g : c->gain) gain_free(&g, s);
+    for (Image &im : c->img) image_free(im, s);
     dev_free(c->flush_buf, s);
     if (c->h2d) (void)cudaStreamDestroy(c->h2d);
     if (c->d2h) (void)cudaStreamDestroy(c->d2h);
@@ -215,9 +222,6 @@ static int crop_image(const sb_crop *crop, int i, const Rect &warped, Rect *proj
     return SB_OK;
 }
 
-// the packed source the warp kernel of image i reads in `sl` (the FINAL-size one of a resized image)
-static const uint8_t *warp_src(const sb_compositor *c, const Slot &sl, int i) { return c->taps_dev[i] ? sl.fin[i] : sl.src[i]; }
-
 // Images.resize_img_by_scaler sizes: the reference resizes camera frames to the FINAL sizes with cv.resize and never
 // scales up (MegapixDownscaler); the staging buffers hold the frames, so they obey the compositor's source limit
 static int check_input_sizes(const sb_rig *rig, const int *in_w, const int *in_h)
@@ -241,56 +245,53 @@ static int check_input_sizes(const sb_rig *rig, const int *in_w, const int *in_h
     return SB_OK;
 }
 
-// The taps of the resized warped images, and which source layout their warp kernel reads: launch_warp chooses
-// its kernel per batch of SB_WARP_BATCH jobs, and reads the word-per-pixel sources only when the RGBM kernel runs and
-// every job of the batch has one (slot_alloc's rule); a resized image gets only the buffer that is read.
-static int plan_resize(sb_compositor *c, cudaStream_t s)
+// The source the warp kernel reads, chosen once per warped image, and the taps of the images resized on the device.
+// launch_warp picks its kernel per batch of SB_WARP_BATCH jobs of `warped`, and only the RGBM kernel reads words: the
+// images of such a batch read words (unless SB_SRC4=0), those of a k_warp_wide batch (a map projection or a 1-px side
+// in the batch) read packed u8x3.  slot_alloc allocates only the buffer that is read.
+static int plan_sources(sb_compositor *c, cudaStream_t s)
 {
-    std::vector<int> t;
+    const char *e = getenv("SB_SRC4");  // SB_SRC4=0: the warp kernel reads the packed 3-byte sources (A/B switch)
+    const bool src4 = !(e && e[0] == '0');
     const std::vector<int> &order = c->warped;
-    std::vector<WarpJob> batch;
+    std::vector<WarpJob> jobs;
+    for (int i : order) jobs.push_back(c->img[i].job);
     for (size_t b = 0; b < order.size(); b += SB_WARP_BATCH) {
-        const size_t end = std::min(b + SB_WARP_BATCH, order.size());
-        batch.clear();
-        for (size_t k = b; k < end; ++k) batch.push_back(c->jobs[order[k]]);
-        bool words = warp_batch_rgbm(batch.data(), (int)batch.size());
-        for (size_t k = b; k < end; ++k) words = words && c->use_src4 && (long long)c->src_w[order[k]] * c->src_h[order[k]] < (1ll << 31);
-        for (size_t k = b; k < end; ++k) {
-            const int i = order[k];
-            const int w = c->src_w[i], h = c->src_h[i];
-            if (c->in_w[i] == w && c->in_h[i] == h) continue;
-            c->warp_src4[i] = words;
-            t.resize((size_t)3 * (w + h));
-            resize_exact_taps(c->in_w[i], w, t.data());
-            resize_exact_taps(c->in_h[i], h, t.data() + (size_t)3 * w);
-            SB_TRY(dev_alloc((void **)&c->taps_dev[i], t.size() * sizeof(int), s));
-            SB_CUDA(cudaMemcpyAsync(c->taps_dev[i], t.data(), t.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-            SB_CUDA(cudaStreamSynchronize(s));  // t is reused by the next image
-        }
+        const int cnt = (int)std::min<size_t>(SB_WARP_BATCH, order.size() - b);
+        const bool words = src4 && warp_batch_rgbm(jobs.data() + b, cnt);
+        for (int k = 0; k < cnt; ++k) c->img[order[b + k]].words = words;
+    }
+    std::vector<int> t;
+    for (int i : order) {
+        Image &im = c->img[i];
+        if (im.in_w == im.w && im.in_h == im.h) continue;
+        t.resize((size_t)3 * (im.w + im.h));
+        resize_exact_taps(im.in_w, im.w, t.data());
+        resize_exact_taps(im.in_h, im.h, t.data() + (size_t)3 * im.w);
+        SB_TRY(dev_alloc((void **)&im.taps, t.size() * sizeof(int), s));
+        SB_CUDA(cudaMemcpyAsync(im.taps, t.data(), t.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+        SB_CUDA(cudaStreamSynchronize(s));  // t is reused by the next image
     }
     return SB_OK;
 }
 
-// After the frames of images [i0, i1) have reached `sl.src` (in the order of stream s): the sources the warp kernel
-// reads -- the repack, or for a resized image k_resize_src in its place, one launch for all of them
+// image i has buffers here: this compositor warps it
+static bool warped_here(const sb_compositor *c, int i) { return c->img[i].rgbm != nullptr; }
+
+// After the frames of images [i0, i1) have reached `sl` (in the order of stream s): the sources the warp kernel reads in
+// their place -- the repack into words, or for a resized image k_resize_src into either layout, one launch for all of them
 static int prepare_sources(sb_compositor *c, const Slot &sl, int i0, int i1, cudaStream_t s)
 {
     c->resize_jobs.clear();
     for (int i = i0; i < i1; ++i) {
-        if (c->taps_dev[i]) {
-            ResizeJob r;
-            r.src = sl.src[i];
-            r.dst4 = sl.src4[i];
-            r.dst3 = sl.fin[i];
-            r.tx = c->taps_dev[i];
-            r.ty = c->taps_dev[i] + (size_t)3 * c->src_w[i];
-            r.sw = c->in_w[i];
-            r.dw = c->src_w[i];
-            r.px = (long long)c->src_w[i] * c->src_h[i];
-            c->resize_jobs.push_back(r);
-        } else if (sl.src4[i]) {
-            SB_TRY(launch_repack_rgbx(sl.src[i], sl.src4[i], (long long)c->src_w[i] * c->src_h[i], s));
-        }
+        const Image &im = c->img[i];
+        const SlotImage &si = sl.img[i];
+        uint32_t *words = im.words ? (uint32_t *)si.src : nullptr;
+        if (im.taps)  // {src, dst4, dst3, tx, ty, sw, dw, px}
+            c->resize_jobs.push_back(ResizeJob{si.frame, words, words ? nullptr : (uint8_t *)si.src, im.taps, im.taps + (size_t)3 * im.w,
+                                               im.in_w, im.w, (long long)im.w * im.h});
+        else if (words)
+            SB_TRY(launch_repack_rgbx(si.frame, words, (long long)im.w * im.h, s));
     }
     return c->resize_jobs.empty() ? SB_OK : launch_resize_src(c->resize_jobs.data(), (int)c->resize_jobs.size(), s);
 }
@@ -321,17 +322,16 @@ static int plan_timelapse(sb_compositor *c, int kind, const int *corners, const 
         set_error("compositor: the timelapse canvas (%d,%d %dx%d) has a zero side", cv.x, cv.y, cv.w, cv.h);
         return SB_ERR_INVALID;
     }
-    c->part.assign(n, Rect{0, 0, 0, 0});
-    c->paste_off.assign(n, 0);
     for (int i = 0; i < n; ++i) {
-        const Rect &r = c->rects[i];
+        Image &im = c->img[i];
+        const Rect &r = im.rect;
         const int x0 = std::max(r.x, cv.x), y0 = std::max(r.y, cv.y);
         const int x1 = std::min(r.x + r.w, cv.x + cv.w), y1 = std::min(r.y + r.h, cv.y + cv.h);
         if (x1 <= x0 || y1 <= y0) continue;
-        c->part[i] = Rect{x0, y0, x1 - x0, y1 - y0};
+        im.part = Rect{x0, y0, x1 - x0, y1 - y0};
         proj[i] = Rect{proj[i].x + x0 - r.x, proj[i].y + y0 - r.y, x1 - x0, y1 - y0};
         const long long bytes = 3ll * (x1 - x0) * (y1 - y0);
-        c->paste_off[i] = c->paste_bytes;
+        im.paste_off = c->paste_bytes;
         c->paste_bytes += ((size_t)bytes + 15) & ~(size_t)15;
         c->paste_max = std::max(c->paste_max, bytes);
         c->paste_model += 7.0 * (x1 - x0) * (y1 - y0);  // RGBM words read, u8x3 written
@@ -355,81 +355,71 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_compos
     SB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     cudaStream_t s = c->stream;
 
-    c->src_w.assign(rig->src_w, rig->src_w + n);
-    c->src_h.assign(rig->src_h, rig->src_h + n);
     if (in_w) SB_TRY(check_input_sizes(rig, in_w, in_h));
-    c->in_w.assign(in_w ? in_w : rig->src_w, (in_w ? in_w : rig->src_w) + n);
-    c->in_h.assign(in_h ? in_h : rig->src_h, (in_h ? in_h : rig->src_h) + n);
-    c->taps_dev.assign(n, nullptr);
-    c->warp_src4.assign(n, 0);
-    c->rects.resize(n);
-    c->jobs.resize(n);
-    {
-        const char *e = getenv("SB_SRC4");  // SB_SRC4=0: the warp kernel reads the packed 3-byte sources (A/B switch)
-        c->use_src4 = !(e && e[0] == '0');
-    }
-    c->rgbm_dev.assign(n, nullptr);
-    c->tab_dev.assign(n, nullptr);
-    c->maps_dev.assign(n, nullptr);
-    c->usermask_dev.assign(n, nullptr);
-    c->gain.assign(n, GainData{});
+    c->img.resize(n);
     std::vector<int> corners(2 * n), sizes(2 * n);
     std::vector<Rect> proj(n);  // the pano-absolute rect image i is warped over
     std::vector<Projector> projs(n);
     for (int i = 0; i < n; ++i) {
+        Image &im = c->img[i];
+        im.w = rig->src_w[i];
+        im.h = rig->src_h[i];
+        im.in_w = in_w ? in_w[i] : im.w;
+        im.in_h = in_h ? in_h[i] : im.h;
         Projector &p = projs[i];
         projector_setup(p, rig->warp_type, rig->scale, rig->K + 9 * i, rig->R + 9 * i);
         int rect[4];
-        projector_roi(p, c->src_w[i], c->src_h[i], rect);
+        projector_roi(p, im.w, im.h, rect);
         if (rect[2] <= 0 || rect[3] <= 0 || (long long)rect[2] * rect[3] > (1ll << 31)) {
             set_error("compositor: degenerate warped roi %dx%d for image %d", rect[2], rect[3], i);
             return SB_ERR_INVALID;
         }
         // the reference warps every image whole (before any crop) with cv::remap, which refuses such sides
-        if (c->src_w[i] >= SB_MAX_WARP_SIDE || c->src_h[i] >= SB_MAX_WARP_SIDE || rect[2] >= SB_MAX_WARP_SIDE || rect[3] >= SB_MAX_WARP_SIDE) {
+        if (im.w >= SB_MAX_WARP_SIDE || im.h >= SB_MAX_WARP_SIDE || rect[2] >= SB_MAX_WARP_SIDE || rect[3] >= SB_MAX_WARP_SIDE) {
             set_error("compositor: image %d (source %dx%d, warped %dx%d) has a side of %d px or more, which cv::remap refuses", i,
-                      c->src_w[i], c->src_h[i], rect[2], rect[3], SB_MAX_WARP_SIDE);
+                      im.w, im.h, rect[2], rect[3], SB_MAX_WARP_SIDE);
             return SB_ERR_INVALID;
         }
-        c->rects[i] = Rect{rect[0], rect[1], rect[2], rect[3]};
+        im.rect = Rect{rect[0], rect[1], rect[2], rect[3]};
         corners[2 * i] = rect[0];
         corners[2 * i + 1] = rect[1];
         sizes[2 * i] = rect[2];
         sizes[2 * i + 1] = rect[3];
-        if (crop) {  // from here on `rect` is the part of the warped rect that is warped and fed, c->rects[i] where it is fed
+        if (crop) {  // from here on `rect` is the part of the warped rect that is warped and fed, im.rect where it is fed
             Rect slice;
-            SB_TRY(crop_image(crop, i, c->rects[i], &slice, &c->rects[i], &sizes[2 * i]));
+            SB_TRY(crop_image(crop, i, im.rect, &slice, &im.rect, &sizes[2 * i]));
             rect[0] = slice.x;
             rect[1] = slice.y;
             rect[2] = slice.w;
             rect[3] = slice.h;
-            corners[2 * i] = c->rects[i].x;
-            corners[2 * i + 1] = c->rects[i].y;
+            corners[2 * i] = im.rect.x;
+            corners[2 * i + 1] = im.rect.y;
         }
         proj[i] = Rect{rect[0], rect[1], rect[2], rect[3]};
     }
     if (c->timelapse) SB_TRY(plan_timelapse(c, c->timelapse, corners.data(), sizes.data(), proj.data()));
     // the images this compositor warps: its block, less those off the timelapse canvas (neither uploaded nor warped)
     for (int i = c->first; i < c->first + c->count; ++i)
-        if (!c->timelapse || c->part[i].w > 0) c->warped.push_back(i);
+        if (!c->timelapse || c->img[i].part.w > 0) c->warped.push_back(i);
     std::vector<float> host_tab;
     for (int i : c->warped) {
+        Image &im = c->img[i];
         const Projector &p = projs[i];
         int rect[4] = {proj[i].x, proj[i].y, proj[i].w, proj[i].h};
-        SB_TRY(dev_alloc((void **)&c->rgbm_dev[i], (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
+        SB_TRY(dev_alloc((void **)&im.rgbm, (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
         // the row padding (never written by the warp kernel) is read by the tile kernels' 16-byte copies: weight 0
-        SB_CUDA(cudaMemsetAsync(c->rgbm_dev[i], 0, (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
-        SB_TRY(dev_alloc((void **)&c->tab_dev[i], warp_table_floats(rect[2], rect[3]) * sizeof(float), s));
-        SB_TRY(make_warp_job(p, rect, c->src_w[i], c->src_h[i], c->tab_dev[i], &c->jobs[i], s, host_tab));
+        SB_CUDA(cudaMemsetAsync(im.rgbm, 0, (size_t)rgbm_pitch_of(rect[2]) * rect[3] * 4, s));
+        SB_TRY(dev_alloc((void **)&im.tab, warp_table_floats(rect[2], rect[3]) * sizeof(float), s));
+        SB_TRY(make_warp_job(p, rect, im.w, im.h, im.tab, &im.job, s, host_tab));
         SB_CUDA(cudaStreamSynchronize(s));  // host_tab is reused by the next image
         if (projector_needs_maps(p)) {
-            SB_TRY(dev_alloc((void **)&c->maps_dev[i], (size_t)2 * rect[2] * rect[3] * sizeof(float), s));
-            SB_TRY(warp_maps_upload(p, rect, c->maps_dev[i], &c->jobs[i], s));
+            SB_TRY(dev_alloc((void **)&im.maps, (size_t)2 * rect[2] * rect[3] * sizeof(float), s));
+            SB_TRY(warp_maps_upload(p, rect, im.maps, &im.job, s));
         }
-        c->jobs[i].spitch = (long long)c->src_w[i] * 3;
-        c->jobs[i].dst_rgbm = c->rgbm_dev[i];
-        c->jobs[i].rgbm_pitch = rgbm_pitch_of(rect[2]);
-        c->warp_bytes += 3.0 * c->src_w[i] * c->src_h[i] + 4.0 * rect[2] * rect[3];
+        im.job.spitch = (long long)im.w * 3;
+        im.job.dst_rgbm = im.rgbm;
+        im.job.rgbm_pitch = rgbm_pitch_of(rect[2]);
+        c->warp_bytes += 3.0 * im.w * im.h + 4.0 * rect[2] * rect[3];
     }
     if (!c->timelapse) {  // a timelapse has no blend plan: its step is warp -> paste into the slot's frames
         // Blender.prepare (blender.py:23-38)
@@ -443,15 +433,15 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_compos
             const char *e = getenv("SB_PD_BIN");
             c->plan.binary_masks = !(e && e[0] == '0');
         }
-        for (int i = 0; i < n; ++i) {
+        for (const Image &im : c->img) {
             FeedDesc f;
             std::memset(&f, 0, sizeof f);
-            f.w = c->rects[i].w;
-            f.h = c->rects[i].h;
-            f.tlx = c->rects[i].x;
-            f.tly = c->rects[i].y;
-            f.rgbm = c->rgbm_dev[i];
-            f.rgbm_pitch = rgbm_pitch_of(c->rects[i].w);
+            f.w = im.rect.w;
+            f.h = im.rect.h;
+            f.tlx = im.rect.x;
+            f.tly = im.rect.y;
+            f.rgbm = im.rgbm;
+            f.rgbm_pitch = rgbm_pitch_of(im.rect.w);
             SB_TRY(c->plan.add_feed(f));
         }
         int out_w = roi.w, out_h = roi.h;
@@ -471,7 +461,7 @@ static int compositor_build(sb_compositor *c, const sb_rig *rig, const sb_compos
         c->slots[0].out.w = out_w;
         c->slots[0].out.h = out_h;
     }
-    SB_TRY(plan_resize(c, s));
+    SB_TRY(plan_sources(c, s));
     SB_TRY(slot_alloc(c, c->slots[0]));
     c->n_slots = 1;
     SB_CUDA(cudaStreamSynchronize(s));
@@ -485,9 +475,11 @@ static const WarpJob *warp_jobs(sb_compositor *c, int slot)
     const Slot &sl = c->slots[slot];
     c->step_jobs.clear();
     for (int i : c->warped) {
-        WarpJob j = c->jobs[i];
-        j.src = warp_src(c, sl, i);
-        j.src4 = sl.src4[i];
+        const Image &im = c->img[i];
+        const SlotImage &si = sl.img[i];
+        WarpJob j = im.job;
+        j.src4 = im.words ? (const uint32_t *)si.src : nullptr;
+        j.src = im.words ? nullptr : im.taps ? (const uint8_t *)si.src : si.frame;
         c->step_jobs.push_back(j);
     }
     return c->step_jobs.data();
@@ -505,13 +497,14 @@ static void drop_graphs(sb_compositor *c)
 #endif
 }
 
-// image i blends with the mask in usermask_dev[i]: stored as its weight byte (and_validity 0) or ANDed with the
+// image i blends with the mask in its usermask: stored as its weight byte (and_validity 0) or ANDed with the
 // warped validity mask (1); the mask may hold gray values
 static void use_blend_mask(sb_compositor *c, int i, int and_validity)
 {
-    c->jobs[i].blend_mask = c->usermask_dev[i];
-    c->jobs[i].blend_mask_pitch = c->rects[i].w;
-    c->jobs[i].blend_mask_and = and_validity;
+    Image &im = c->img[i];
+    im.job.blend_mask = im.usermask;
+    im.job.blend_mask_pitch = im.rect.w;
+    im.job.blend_mask_and = and_validity;
     c->plan.binary_masks = false;
     drop_graphs(c);
 }
@@ -779,7 +772,7 @@ static int pipe_step(sb_compositor *c, const char *what, const uint8_t *const *s
                      const std::function<int(const Slot &)> &download, unsigned long long *ticket)
 {
     for (int i = 0; i < c->n; ++i)
-        if (!srcs[i] || pitches[i] < (size_t)c->in_w[i] * 3) {
+        if (!srcs[i] || pitches[i] < (size_t)c->img[i].in_w * 3) {
             set_error("%s: invalid source %d", what, i);
             return SB_ERR_INVALID;
         }
@@ -792,9 +785,10 @@ static int pipe_step(sb_compositor *c, const char *what, const uint8_t *const *s
     // (download() is synchronous, so the output buffers need no such guard)
     if (t < SB_PIPE_DEPTH) SB_CUDA(cudaEventRecord(sl.e_comp, c->stream));
     SB_CUDA(cudaStreamWaitEvent(c->h2d, sl.e_comp, 0));
-    for (int i : c->warped)
-        SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->in_w[i] * 3, srcs[i], pitches[i], (size_t)c->in_w[i] * 3, c->in_h[i],
-                          cudaMemcpyHostToDevice, c->h2d));
+    for (int i : c->warped) {
+        const Image &im = c->img[i];
+        SB_CUDA(sb_copy2d(sl.img[i].frame, (size_t)im.in_w * 3, srcs[i], pitches[i], (size_t)im.in_w * 3, im.in_h, cudaMemcpyHostToDevice, c->h2d));
+    }
     // the repack (and resize) kernels follow the LAST copy (same stream): a kernel between two copies would leave the PCIe
     // link idle for its launch + run time, eight times per step
     SB_TRY(prepare_sources(c, sl, 0, c->n, c->h2d));
@@ -925,10 +919,10 @@ int sb_compositor_geometry(const sb_compositor *c, int *rects, int pano_roi[4], 
     }
     if (rects)
         for (int i = 0; i < c->n; ++i) {
-            rects[4 * i] = c->rects[i].x;
-            rects[4 * i + 1] = c->rects[i].y;
-            rects[4 * i + 2] = c->rects[i].w;
-            rects[4 * i + 3] = c->rects[i].h;
+            rects[4 * i] = c->img[i].rect.x;
+            rects[4 * i + 1] = c->img[i].rect.y;
+            rects[4 * i + 2] = c->img[i].rect.w;
+            rects[4 * i + 3] = c->img[i].rect.h;
         }
     if (pano_roi) {
         const Rect &r = c->timelapse ? c->canvas : c->plan.roi;  // a timelapse: its canvas
@@ -964,18 +958,17 @@ int sb_compositor_model_bytes(const sb_compositor *c, double *total_bytes, doubl
 int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pitch, int pinned)
 {
     if (refuse_timelapse(c, "sb_compositor_upload")) return SB_ERR_STATE;
-    if (!c || i < 0 || i >= c->n || !src || pitch < (size_t)c->in_w[i] * 3) {
+    if (!c || i < 0 || i >= c->n || !src || pitch < (size_t)c->img[i].in_w * 3) {
         set_error("sb_compositor_upload: invalid argument");
         return SB_ERR_INVALID;
     }
-    const Slot &sl = c->slots[0];
-    if (!sl.src[i]) {
+    if (!warped_here(c, i)) {
         set_error("sb_compositor_upload: image %d belongs to another rank (this rank owns %d..%d)", i, c->first, c->first + c->count - 1);
         return SB_ERR_INVALID;
     }
-    SB_CUDA(sb_copy2d(sl.src[i], (size_t)c->in_w[i] * 3, src, pitch, (size_t)c->in_w[i] * 3, c->in_h[i], cudaMemcpyHostToDevice,
-                      c->stream));
-    SB_TRY(prepare_sources(c, sl, i, i + 1, c->stream));
+    const Image &im = c->img[i];
+    SB_CUDA(sb_copy2d(c->slots[0].img[i].frame, (size_t)im.in_w * 3, src, pitch, (size_t)im.in_w * 3, im.in_h, cudaMemcpyHostToDevice, c->stream));
+    SB_TRY(prepare_sources(c, c->slots[0], i, i + 1, c->stream));
     if (!pinned) SB_CUDA(cudaStreamSynchronize(c->stream));
     return SB_OK;
 }
@@ -983,15 +976,16 @@ int sb_compositor_upload(sb_compositor *c, int i, const uint8_t *src, size_t pit
 int sb_compositor_set_mask(sb_compositor *c, int i, const uint8_t *mask, size_t pitch)
 {
     if (refuse_timelapse(c, "sb_compositor_set_mask")) return SB_ERR_STATE;  // the Timelapser ignores masks
-    if (!c || i < 0 || i >= c->n || !mask || pitch < (size_t)c->rects[i].w || !c->rgbm_dev[i]) {
+    if (!c || i < 0 || i >= c->n || !mask || pitch < (size_t)c->img[i].rect.w || !warped_here(c, i)) {
         set_error("sb_compositor_set_mask: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
     }
     // the blend mask of image i in warped coordinates (what stitcher.py:223-239 hands to Blender.feed); it replaces
     // the validity mask in the weight byte of the packed warped image from the next run on
-    const int w = c->rects[i].w, h = c->rects[i].h;
-    if (!c->usermask_dev[i]) SB_TRY(dev_alloc((void **)&c->usermask_dev[i], (size_t)w * h, c->stream));
-    SB_CUDA(sb_copy2d(c->usermask_dev[i], w, mask, pitch, w, h, cudaMemcpyHostToDevice, c->stream));
+    Image &im = c->img[i];
+    const int w = im.rect.w, h = im.rect.h;
+    if (!im.usermask) SB_TRY(dev_alloc((void **)&im.usermask, (size_t)w * h, c->stream));
+    SB_CUDA(sb_copy2d(im.usermask, w, mask, pitch, w, h, cudaMemcpyHostToDevice, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
     use_blend_mask(c, i, 0);
     return SB_OK;
@@ -1000,40 +994,42 @@ int sb_compositor_set_mask(sb_compositor *c, int i, const uint8_t *mask, size_t 
 int sb_compositor_set_seam_mask(sb_compositor *c, int i, const uint8_t *seam, size_t seam_pitch, int sw, int sh)
 {
     if (refuse_timelapse(c, "sb_compositor_set_seam_mask")) return SB_ERR_STATE;
-    if (!c || i < 0 || i >= c->n || !seam || sw <= 0 || sh <= 0 || seam_pitch < (size_t)sw || !c->rgbm_dev[i]) {
+    if (!c || i < 0 || i >= c->n || !seam || sw <= 0 || sh <= 0 || seam_pitch < (size_t)sw || !warped_here(c, i)) {
         set_error("sb_compositor_set_seam_mask: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
     }
     // SeamFinder.resize(seam_mask, warped mask) (seam_finder.py:38-43, stitcher.py:223-225) without the host round
     // trip: the LOW-resolution seam mask is dilated and resized on the device; the AND with the warped validity mask
     // happens in the warp kernel, which computes that mask anyway
-    const int w = c->rects[i].w, h = c->rects[i].h;
-    if (!c->usermask_dev[i]) SB_TRY(dev_alloc((void **)&c->usermask_dev[i], (size_t)w * h, c->stream));
-    SB_TRY(seam_resize_device(seam, seam_pitch, sw, sh, nullptr, 0, c->usermask_dev[i], w, w, h, c->stream));
+    Image &im = c->img[i];
+    const int w = im.rect.w, h = im.rect.h;
+    if (!im.usermask) SB_TRY(dev_alloc((void **)&im.usermask, (size_t)w * h, c->stream));
+    SB_TRY(seam_resize_device(seam, seam_pitch, sw, sh, nullptr, 0, im.usermask, w, w, h, c->stream));
     use_blend_mask(c, i, 1);
     return SB_OK;
 }
 
 int sb_compositor_set_gain(sb_compositor *c, int i, const float *gain_map, int gw, int gh, int gc, const double *gain_scalar)
 {
-    if (!c || i < 0 || i >= c->n || (!c->rgbm_dev[i] && !c->timelapse) || (gain_map && gain_scalar) ||
+    if (!c || i < 0 || i >= c->n || (!warped_here(c, i) && !c->timelapse) || (gain_map && gain_scalar) ||
         (gain_map && (gw <= 0 || gh <= 0 || (gc != 1 && gc != 3)))) {
         set_error("sb_compositor_set_gain: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
     }
-    if (!c->rgbm_dev[i]) return SB_OK;  // off the timelapse canvas: nothing of it is shown
+    if (!warped_here(c, i)) return SB_OK;  // off the timelapse canvas: nothing of it is shown
     // ExposureErrorCompensator.apply(i, corner, warped image, mask) (exposure_error_compensator.py:43-45,
     // stitcher.py:219-221) fused into the warp's epilogue: the warped image never exists uncompensated
     SB_CUDA(cudaStreamSynchronize(c->stream));  // the previous run may still read the old gain buffers
     drop_graphs(c);  // before the upload, which frees the buffers they read
-    const Rect &r = c->rects[i];
+    Image &im = c->img[i];
+    const Rect &r = im.rect;
     if (c->timelapse) {
         // only P_i is warped, but the gain map is resized to the whole fed image: the taps at P_i's place in it
-        const Rect &p = c->part[i];
+        const Rect &p = im.part;
         const int sub[4] = {p.x - r.x, p.y - r.y, p.w, p.h};
-        return gain_upload(&c->jobs[i], &c->gain[i], r.w, r.h, gain_map, gw, gh, gc, gain_scalar, c->stream, sub);
+        return gain_upload(&im.job, &im.gain, r.w, r.h, gain_map, gw, gh, gc, gain_scalar, c->stream, sub);
     }
-    return gain_upload(&c->jobs[i], &c->gain[i], r.w, r.h, gain_map, gw, gh, gc, gain_scalar, c->stream);
+    return gain_upload(&im.job, &im.gain, r.w, r.h, gain_map, gw, gh, gc, gain_scalar, c->stream);
 }
 
 int sb_compositor_run(sb_compositor *c)
@@ -1108,9 +1104,9 @@ int sb_compositor_submit_timelapse(sb_compositor *c, const uint8_t *const *srcs,
         const Rect &cv = c->canvas;
         const size_t fpitch = (size_t)cv.w * 3, fbytes = fpitch * cv.h;
         for (int i : c->warped) {
-            const Rect &p = c->part[i];
+            const Rect &p = c->img[i].part;
             uint8_t *dst = sl.frames + fbytes * i + (size_t)(p.y - cv.y) * fpitch + (size_t)(p.x - cv.x) * 3;
-            SB_CUDA(sb_copy2d(dst, fpitch, sl.paste + c->paste_off[i], (size_t)p.w * 3, (size_t)p.w * 3, p.h, cudaMemcpyDeviceToHost, c->d2h));
+            SB_CUDA(sb_copy2d(dst, fpitch, sl.paste + c->img[i].paste_off, (size_t)p.w * 3, (size_t)p.w * 3, p.h, cudaMemcpyDeviceToHost, c->d2h));
         }
         return SB_OK;
     };
@@ -1135,14 +1131,14 @@ int sb_compositor_timelapse_frame(const sb_compositor *c, unsigned long long tic
 int sb_compositor_download_warped(sb_compositor *c, int i, uint8_t *dst, size_t dst_pitch, uint8_t *dst_mask, size_t mask_pitch)
 {
     if (refuse_timelapse(c, "sb_compositor_download_warped")) return SB_ERR_STATE;
-    if (!c || i < 0 || i >= c->n || !c->rgbm_dev[i]) {
+    if (!c || i < 0 || i >= c->n || !warped_here(c, i)) {
         set_error("sb_compositor_download_warped: invalid argument (or an image of another rank)");
         return SB_ERR_INVALID;
     }
-    const int w = c->rects[i].w, h = c->rects[i].h;
+    const int w = c->img[i].rect.w, h = c->img[i].rect.h;
     const size_t wp = (size_t)rgbm_pitch_of(w);
     std::vector<uint32_t> tmp(wp * h);
-    SB_CUDA(cudaMemcpyAsync(tmp.data(), c->rgbm_dev[i], tmp.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+    SB_CUDA(cudaMemcpyAsync(tmp.data(), c->img[i].rgbm, tmp.size() * 4, cudaMemcpyDeviceToHost, c->stream));
     SB_CUDA(cudaStreamSynchronize(c->stream));
     for (int y = 0; y < h; ++y)
         for (int x = 0; x < w; ++x) {

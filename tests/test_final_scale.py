@@ -30,8 +30,8 @@ def test_resize_kernel_against_oracle(use_emu, oracle, k):
 
 
 def test_resize_kernel_packed_output(use_emu, oracle, monkeypatch):
-    """SB_SRC4=0: the kernel writes the packed FINAL source instead of words.  (The other case in which a compositor
-    has no word source, an image of 2^31 px or more, cannot occur: sources are below 32767 px a side.)"""
+    """SB_SRC4=0: the kernel writes the packed FINAL source instead of words for every image, not only for those in a
+    batch that k_warp_wide warps."""
     monkeypatch.setenv("SB_SRC4", "0")
     final_scale.kernel_check(oracle, _kernel_rig(1), SEED + 100)
 

@@ -59,7 +59,7 @@ def test_compositor_matches_oracle(use_emu, oracle):
 
 
 def test_source_layouts_of_the_warp_kernel_agree(use_emu, monkeypatch):
-    """The compositor repacks every uploaded source to one word per pixel for the warp kernel (SB_SRC4, default on); the
+    """The compositor repacks the uploaded sources of a spherical rig to one word per pixel for the warp kernel (SB_SRC4, default on); the
     packed 3-byte path (SB_SRC4=0) is the same arithmetic on the same pixels: identical panoramas, masks and warped images."""
     cfg = rigs.config("cfg2", 16)
     cams = cfg["cameras"][:4]
@@ -76,6 +76,31 @@ def test_source_layouts_of_the_warp_kernel_agree(use_emu, monkeypatch):
     replay.assert_exact(out[0][1], out[1][1], "mask, word-per-pixel vs packed sources")
     for a, b in zip(out[0][2], out[1][2]):
         assert np.array_equal(a, b)
+
+
+def test_upload_prepares_only_the_source_the_warp_reads(use_emu, oracle):
+    """The source layout of an image is chosen once, per batch of warp jobs: an upload on a map-projection rig launches no
+    kernel (k_warp_wide reads the frame as uploaded), on a spherical rig one repack per image (k_warp_rgbm reads words), and
+    with input_sizes one k_resize_src per batch of resized images, whichever layout it writes (Compositor.upload uploads
+    one image per call: one launch per image).  The panoramas equal the oracle's; the camera frames are the images at
+    twice the size, which resize back to them exactly."""
+    cfg = rigs.config("cfg2", 25)
+    cams = cfg["cameras"][2:5]
+    sizes = [(cfg["w"], cfg["h"])] * len(cams)
+    imgs = [rigs.noise_image(cfg["h"], cfg["w"], 3000 + i) for i in range(len(cams))]
+    frames = [np.ascontiguousarray(im.repeat(2, 0).repeat(2, 1)) for im in imgs]
+    for warper, repacks in (("fisheye", 0), ("spherical", len(cams))):
+        ref = replay.oracle_composite(oracle, dict(cfg, warper=warper), cams, imgs)
+        for input_sizes, uploaded, launches in ((None, imgs, repacks), ([(2 * w, 2 * h) for w, h in sizes], frames, len(cams))):
+            c = Compositor(cams, sizes, warper, cfg["blender"], cfg["strength"], input_sizes=input_sizes)
+            before = use_emu.sb_launch_count()
+            c.upload(uploaded)
+            assert use_emu.sb_launch_count() - before == launches, (warper, input_sizes)
+            c.run()
+            pano, mask = c.download()
+            c.close()
+            replay.assert_exact(pano, ref["pano"], f"{warper} pano, input sizes {input_sizes}")
+            replay.assert_exact(mask, ref["pmask"], f"{warper} mask, input sizes {input_sizes}")
 
 
 def test_host_pool_reuses_and_bounds_page_locked_memory(use_emu, monkeypatch):
