@@ -3,6 +3,7 @@ in one process on one library: tests/test_emu_memory.py runs it in child process
 allocations start filled with a byte (SB_EMU_FILL) and on the same sources under AddressSanitizer + UBSan.
 
     python tests/emu_sweep.py --lib tests/emu/libstitch_b200_emu.so [--corpora rig_fuzz,crop_fuzz]
+    python tests/emu_sweep.py --lib <mutant>.so --cases rig_fuzz:case_3,kernel_edges:gain_2p31
 
 Each case is one call of an existing test function with its parameters (its env set as the test sets it, through a
 MonkeyPatch undone after the case); a case passes when the call returns.  Prints one line per corpus with its number of
@@ -24,6 +25,7 @@ def corpora(L, O):
     oracle module."""
     import crop_fuzz
     import dropin_fuzz
+    import kernel_edges
     import rig_fuzz
     import shard_fuzz
     import test_crop
@@ -67,15 +69,17 @@ def corpora(L, O):
         "lanes_blocks": [("lanes_shuffle_pyrdown", lambda mp: H.test_warp_collective_kernels_under_lane_emulation(L, O, mp)),
                          ("blocks_tile_collapse", lambda mp: H.test_shared_memory_tile_kernels_under_block_emulation(L, O, mp)),
                          ("lanes_distance_transform", lambda mp: H.test_parallel_distance_transform_under_lane_emulation(L, O, mp))],
+        "kernel_edges": [(cid, lambda mp, fn=fn: fn(O, mp)) for cid, fn in kernel_edges.emu_cases()],
     }
 
 
 NAMES = ["rig_fuzz", "crop_fuzz", "shard_fuzz", "dropin_fuzz", "final_scale", "timelapse_fuzz", "fullres", "goldens",
-         "setters", "lanes_blocks"]
+         "setters", "lanes_blocks", "kernel_edges"]
 
 
-def run(lib_path, names, out=sys.stdout):
-    """Run the named corpora on the library at lib_path; returns {corpus: (cases, [(case id, message)])}."""
+def run(lib_path, names, out=sys.stdout, only=None):
+    """Run the named corpora on the library at lib_path; returns {corpus: (cases, [(case id, message)])}.  `only`: a set
+    of "corpus:case id" to run instead of whole corpora."""
     import pytest
 
     from oracle import oracle as O
@@ -88,6 +92,8 @@ def run(lib_path, names, out=sys.stdout):
     res = {}
     for name in names:
         cases, failed, t0 = table[name], [], time.time()
+        if only is not None:
+            cases = [(cid, fn) for cid, fn in cases if f"{name}:{cid}" in only]
         for cid, fn in cases:
             with pytest.MonkeyPatch.context() as mp:
                 try:
@@ -106,15 +112,23 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--lib", default=os.path.join(ROOT, "tests", "emu", "libstitch_b200_emu.so"))
     ap.add_argument("--corpora", default=",".join(NAMES))
+    ap.add_argument("--cases", default="", help="comma-separated corpus:case ids (replaces --corpora)")
     a = ap.parse_args()
     names = [n for n in a.corpora.split(",") if n]
+    only = None
+    if a.cases:
+        only = {c for c in a.cases.split(",") if c}
+        names = [n for n in NAMES if any(c.split(":", 1)[0] == n for c in only)]
     unknown = sorted(set(names) - set(NAMES))
     if unknown:
         ap.error(f"unknown corpora {unknown}; known: {NAMES}")
     print(f"sweep on {a.lib}, SB_EMU_FILL={os.environ.get('SB_EMU_FILL', '(unset)')}", flush=True)
-    res = run(a.lib, names)
+    res = run(a.lib, names, only=only)
     total = sum(n for n, _ in res.values())
     bad = sum(len(f) for _, f in res.values())
+    if only is not None and total != len(only):
+        print(f"unknown cases: {total} of {len(only)} found", flush=True)
+        bad += 1
     print(f"all corpora: {total} cases, {bad} failed", flush=True)
     sys.exit(1 if bad else 0)
 

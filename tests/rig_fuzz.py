@@ -320,12 +320,24 @@ def named(name, budget):
         gains[WARP_BATCH + 1] = "map3"
         c = Case(name, "affine", cams, sizes, "multiband", 0.0, masks, gains, ["noise"] * n, 14)
     elif name == "odd_origins":
-        # rects at odd origins and an odd pano width: the tile kernel's level 0 declines (sb_collapse_tile.cu:555)
+        # rects at odd origins and an odd pano width: the tile kernel's level 0 declines (launch_collapse_tile: odd
+        # output pitches)
         sizes = [(min(side, 61), min(side, 45)), (min(side, 53), min(side, 47)), (min(side, 40), min(side, 31))]
         cams = [rigs.Camera(1, 1, 0, 0, np.array([[1, 0, 3.7], [0, 1, 1.3], [0, 0, 1]], np.float32)),
                 rigs.Camera(1, 1, 0, 0, np.array([[0.95, 0.1, 37.2], [-0.1, 1.05, 9.6], [0, 0, 1]], np.float32)),
                 rigs.Camera(1, 1, 0, 0, np.array([[1, 0, 19.5], [0, 1, 33.9], [0, 0, 1]], np.float32))]
         c = Case(name, "affine", cams, sizes, "multiband", 0.0, ["none", "seam", "none"], ["none"] * 3, ["synth", "noise", "noise"], 15)
+    elif name in ("thin_w", "thin_h"):
+        # a pano 4 px wide (thin_w) or high (thin_h) with two bands: every padded rect is one 4-px lattice cell across,
+        # so level 2 is 1 px wide (high) and k_collapse_tile's level 1 stages a coarse window of one column (row):
+        # fix_borders' reflect-101 of a 1-px level
+        sizes = [(4, min(side, 40)), (4, min(side, 37))]
+        offs = [(0.0, 0.0), (0.0, 23.0)]
+        if name == "thin_h":
+            sizes = [(h, w) for w, h in sizes]
+            offs = [(y, x) for x, y in offs]
+        cams = [rigs.Camera(1, 1, 0, 0, np.array([[1, 0, ox], [0, 1, oy], [0, 0, 1]], np.float32)) for ox, oy in offs]
+        c = Case(name, "affine", cams, sizes, "multiband", 0.0, ["none", "ramp"], ["none"] * 2, ["noise", "synth"], 17)
     elif name == "wide_feather":
         # a feather image wider than 8192 px: the two-sweep distance-transform row kernel (sb_feather_fast.cu:271-272)
         sizes = [(8300, 9), (700, 60)]
@@ -346,9 +358,9 @@ LANES, BLOCKS = {"SB_EMU_LANES": "1"}, {"SB_EMU_BLOCKS": "1"}
 EMU_COUNT = 36
 # emulation: the shuffle pyrDown runs only under SB_EMU_LANES and the tile collapse only under SB_EMU_BLOCKS (slow)
 EMU_NAMED = [("flat_top", LANES), ("gray_mask_multiband", LANES), ("thin_levels", LANES),
-             ("odd_origins", BLOCKS), ("many", BLOCKS), ("gray_mask_multiband", BLOCKS)]
+             ("odd_origins", BLOCKS), ("many", BLOCKS), ("gray_mask_multiband", BLOCKS), ("thin_w", BLOCKS), ("thin_h", BLOCKS)]
 GPU_COUNT = 200
-GPU_NAMED = ["many", "wide_feather", "flat_top", "thin_levels", "odd_origins", "gray_mask_multiband"]
+GPU_NAMED = ["many", "wide_feather", "flat_top", "thin_levels", "odd_origins", "gray_mask_multiband", "thin_w", "thin_h"]
 
 
 def emu_ids():
@@ -543,11 +555,18 @@ def coverage(case, pyr_fast=True, tile=True, dt_fast=True, pd_bin=True):
                 inst = (0, int(near), 0)
             tags.add("k_pyrdown_walk<%d,%d,%d>" % inst)
     if kind == "multiband" and tile and nb >= 1:
-        # tile_images_ok (sb_plan.cpp:319-321) holds for every compositor; launch_collapse_tile (sb_collapse_tile.cu:
-        # 551-557) at level 0 wants even output pitches: 3 * pano width and the mask pitch
+        # tile_images_ok (BlendPlan) holds for every compositor; launch_collapse_tile at level 0 wants even output
+        # pitches: 3 * pano width and the mask pitch
         tags.add("tile l0 yes" if w % 2 == 0 else "tile l0 no")
         if nb >= 2:
             tags.add("tile l1 yes")
+        # the coarse windows a tile level stages (level l + 1 of each image and of the pano) one element across:
+        # fix_borders' reflect-101 of a 1-px level
+        for up in [l + 1 for l in (0, 1) if l < nb and (l == 1 or w % 2 == 0)]:
+            if any(p["pw"] >> up == 1 for p in padded) or -(-w // (1 << nb)) * (1 << nb) >> up == 1:
+                tags.add("tile coarse 1 px wide")
+            if any(p["ph"] >> up == 1 for p in padded) or -(-h // (1 << nb)) * (1 << nb) >> up == 1:
+                tags.add("tile coarse 1 px high")
     if kind == "feather" and max(r[2] for r in case.rects) > 8192:
         tags.add("feather w>8192")
         if dt_fast:
