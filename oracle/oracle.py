@@ -69,6 +69,7 @@ def lib():
         L.so_sb_fold.argtypes = [C.c_void_p, C.c_void_p]
         L.so_convert_scale_abs_s16.argtypes = [s16p, C.c_size_t, u8p]
         L.so_resize_linear_f32.argtypes = [fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, fp]
+        L.so_resize_linear_f32_rule.argtypes = [fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, fp]
         L.so_resize_linear_exact_u8.argtypes = [u8p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, u8p]
         L.so_gain_apply_blocks.argtypes = [u8p, C.c_size_t, C.c_int, C.c_int, fp, C.c_int, C.c_int, C.c_int]
         L.so_gain_apply_scalar.argtypes = [u8p, C.c_size_t, C.c_int, C.c_int, C.POINTER(C.c_double)]
@@ -226,13 +227,19 @@ def resize_linear_exact(a, size):
     return out
 
 
-def resize_linear_f32(a, size):
-    """cv.resize(a, size, interpolation=cv.INTER_LINEAR) for a float32 image of 1 or 3 channels; size = (w, h)."""
+def resize_linear_f32(a, size, rule=None):
+    """cv.resize(a, size, interpolation=cv.INTER_LINEAR) for a float32 image of 1 or 3 channels; size = (w, h).  rule
+    "ipp" or "generic" forces one of the two kernels cv2 picks by the shape (IPP's for both sides >= 2, OpenCV's own for a
+    side of 1): the tests use the rule cv2 does not pick as a foil."""
     a = np.ascontiguousarray(a, np.float32)
     h, w = a.shape[:2]
     cn = 1 if a.ndim == 2 else a.shape[2]
     out = np.empty((int(size[1]), int(size[0])) + (() if a.ndim == 2 else (cn,)), np.float32)
-    lib().so_resize_linear_f32(_p(a, C.c_float), w, h, cn, int(size[0]), int(size[1]), _p(out, C.c_float))
+    if rule is None:
+        lib().so_resize_linear_f32(_p(a, C.c_float), w, h, cn, int(size[0]), int(size[1]), _p(out, C.c_float))
+    else:
+        assert rule in ("ipp", "generic"), rule
+        lib().so_resize_linear_f32_rule(_p(a, C.c_float), w, h, cn, int(size[0]), int(size[1]), int(rule == "generic"), _p(out, C.c_float))
     return out
 
 

@@ -930,31 +930,64 @@ SO_API void so_seam_resize(const uint8_t *seam, size_t seam_pitch, int sw, int s
  *   gain_blocks / channel_blocks (Blocks*Compensator::apply): the float32 gain map (1 or 3 channels, one sample per
  *     block) is resized to the image size with cv::resize(INTER_LINEAR) and multiplied in:
  *         image = saturate_cast<uchar>(cvRound(float(image) * gain))            (float32 product, half to even)
- *     In the reference's wheel that float32 resize runs IPP's kernel, not OpenCV's own; found by hypothesis testing
- *     (0 mismatches, cv2 4.13 with IPP on):  f = (d + 0.5) * (n_src / n_dst) - 0.5 in double, i0 = floor(f),
- *     fraction = float(f - i0), zero where the index is clamped (both axes); horizontal pass first, each pass
- *     a + (b - a) * t as ONE fused multiply-add.
+ *     In the reference's wheel that float32 resize runs one of two kernels, chosen by the map's shape (both rules found
+ *     by hypothesis testing against cv2 4.13 and pinned by tests/golden/gen_gain_map_golden.py -> golden_gain_maps.npz):
+ *     - both sides >= 2: IPP's kernel (bit for bit on 17 of 17 probe shapes, among them downscales, 1-px
+ *       destinations, identity sizes and 2x2 -> 5000x5000):  f = (d + 0.5) * (n_src / n_dst) - 0.5 in double,
+ *       i0 = floor(f), fraction = float(f - i0), zero where the index is clamped (both axes); horizontal pass first,
+ *       each pass a + (b - a) * t as ONE fused multiply-add.
+ *     - a side of 1 (1 x k, k x 1, 1 x 1): OpenCV's own resizeGeneric_, IPP on or off (bit for bit in 60 of 60
+ *       random maps of 1 and 3 channels and destinations up to 2000 x 1200; the IPP rule got 4-47 % of the values
+ *       wrong on such maps, and even a constant 1 x 1 map does not stay constant):  f = float((d + 0.5) *
+ *       (1 / (n_dst / n_src)) - 0.5), i0 = floor(f), fraction f - i0 in float; columns clamp the index and zero the
+ *       fraction at both ends, rows keep the fraction and clamp both indices (a 1-row map gives a (1 - t) + a t);
+ *       horizontal pass first, each pass a (1 - t) + b t as two rounded products and one rounded sum, 1 - t in float.
+ *       Non-finite samples: a left-clamped column is a * 1 + b * 0 with b the sample right of a, as in cv2 (so an inf
+ *       there gives NaN); at a right-clamped column cv2 takes a * 1 alone, where this computes a * 1 + a * 0: NaN
+ *       instead of +-inf when a is not finite, and both round to the byte 0 in apply.
  *   gain / channel (GainCompensator / ChannelsCompensator::apply): a double scalar per image (per channel):
  *         image = saturate_cast<uchar>(cvRound(double(image) * gain))           (double product)
  *   no: identity.
  * Pinned against the reference class (gains estimated by its own feed()) by tests/golden/gen_golden.py -> golden_gain.npz.
  * ---------------------------------------------------------------------------------------- */
-static void resize_f32_taps(int n_src, int n_dst, int *i0, int *i1, float *fr)
+/* the taps of one axis: IPP's (generic = 0), or OpenCV's own for columns (generic = 1) or rows (generic = 2) */
+static void resize_f32_taps(int n_src, int n_dst, int generic, int *i0, int *i1, float *fr)
 {
-    const double scale = (double)n_src / (double)n_dst;
+    const double scale = (double)n_src / (double)n_dst, inv = 1.0 / ((double)n_dst / (double)n_src);
     for (int d = 0; d < n_dst; ++d) {
-        const double f = ((double)d + 0.5) * scale - 0.5;
-        int s = (int)floor(f);
-        float t = (float)(f - (double)s);
-        if (s < 0 || s >= n_src - 1) t = 0.f;
+        int s;
+        float t;
+        if (!generic) {
+            const double f = ((double)d + 0.5) * scale - 0.5;
+            s = (int)floor(f);
+            t = (float)(f - (double)s);
+            if (s < 0 || s >= n_src - 1) t = 0.f;
+        } else {
+            const float f = (float)(((double)d + 0.5) * inv - 0.5);
+            s = (int)floorf(f);
+            t = f - (float)s;
+            if (generic == 1 && (s < 0 || s >= n_src - 1)) {
+                t = 0.f;
+                if (s < 0) s = 0; /* the left end reads sample 0 and its neighbour (weights 1 and 0), as cv2 does */
+            }
+        }
         i0[d] = s < 0 ? 0 : (s > n_src - 1 ? n_src - 1 : s);
         i1[d] = s + 1 < 0 ? 0 : (s + 1 > n_src - 1 ? n_src - 1 : s + 1);
         fr[d] = t;
     }
 }
 
+/* the float32 resize with the rule given: IPP's (generic = 0) or OpenCV's own (1), whatever the map's shape (the
+ * tests use the other rule as a foil) */
+SO_API void so_resize_linear_f32_rule(const float *src, int sw, int sh, int cn, int dw, int dh, int generic, float *dst);
+
 /* cv.resize(float32, cn channels interleaved, INTER_LINEAR) as this wheel computes it */
 SO_API void so_resize_linear_f32(const float *src, int sw, int sh, int cn, int dw, int dh, float *dst)
+{
+    so_resize_linear_f32_rule(src, sw, sh, cn, dw, dh, sw == 1 || sh == 1, dst); /* a side of 1: OpenCV's own kernel */
+}
+
+SO_API void so_resize_linear_f32_rule(const float *src, int sw, int sh, int cn, int dw, int dh, int generic, float *dst)
 {
     if (sw == dw && sh == dh) {
         memcpy(dst, src, sizeof(float) * (size_t)sw * sh * cn);
@@ -962,16 +995,25 @@ SO_API void so_resize_linear_f32(const float *src, int sw, int sh, int cn, int d
     }
     int *x0 = (int *)malloc(sizeof(int) * 2 * (size_t)dw), *y0 = (int *)malloc(sizeof(int) * 2 * (size_t)dh);
     float *fx = (float *)malloc(sizeof(float) * (size_t)dw), *fy = (float *)malloc(sizeof(float) * (size_t)dh);
-    resize_f32_taps(sw, dw, x0, x0 + dw, fx);
-    resize_f32_taps(sh, dh, y0, y0 + dh, fy);
+    resize_f32_taps(sw, dw, generic ? 1 : 0, x0, x0 + dw, fx);
+    resize_f32_taps(sh, dh, generic ? 2 : 0, y0, y0 + dh, fy);
     for (int y = 0; y < dh; ++y) {
         const float *r0 = src + (size_t)y0[y] * sw * cn, *r1 = src + (size_t)y0[dh + y] * sw * cn;
+        const float ty = fy[y], uy = 1.f - ty;
         for (int x = 0; x < dw; ++x)
             for (int c = 0; c < cn; ++c) {
                 const float a0 = r0[x0[x] * cn + c], b0 = r0[x0[dw + x] * cn + c];
                 const float a1 = r1[x0[x] * cn + c], b1 = r1[x0[dw + x] * cn + c];
-                const float h0 = fmaf(b0 - a0, fx[x], a0), h1 = fmaf(b1 - a1, fx[x], a1);
-                dst[((size_t)y * dw + x) * cn + c] = fmaf(h1 - h0, fy[y], h0);
+                const float tx = fx[x], ux = 1.f - tx;
+                float v;
+                if (generic) { /* -ffp-contract=off: every product and sum rounded */
+                    const float h0 = a0 * ux + b0 * tx, h1 = a1 * ux + b1 * tx;
+                    v = h0 * uy + h1 * ty;
+                } else {
+                    const float h0 = fmaf(b0 - a0, tx, a0), h1 = fmaf(b1 - a1, tx, a1);
+                    v = fmaf(h1 - h0, ty, h0);
+                }
+                dst[((size_t)y * dw + x) * cn + c] = v;
             }
     }
     free(x0);

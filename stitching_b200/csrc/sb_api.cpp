@@ -314,8 +314,10 @@ int gain_upload(WarpJob *job, GainData *gd, int w, int h, const float *gain_map,
     if (!gain_map) return SB_OK;  // no gain: compensator "no"
     std::vector<int> tx((size_t)2 * w), ty((size_t)2 * h);
     std::vector<float> fx((size_t)w), fy((size_t)h);
-    resize_f32_taps(gw, w, tx.data(), fx.data());
-    resize_f32_taps(gh, h, ty.data(), fy.data());
+    // cv::resize runs IPP's kernel on a map with both sides >= 2 and OpenCV's own on a map with a side of 1
+    const bool generic = gw == 1 || gh == 1;
+    resize_f32_taps(gw, w, tx.data(), fx.data(), generic ? TAPS_COLS : TAPS_IPP);
+    resize_f32_taps(gh, h, ty.data(), fy.data(), generic ? TAPS_ROWS : TAPS_IPP);
     if (sub) {
         // the taps of columns [x, x + w') and rows [y, y + h') of the whole image: [i0 | i1] halves cut alike
         auto cut = [](std::vector<int> &t, std::vector<float> &f, int n, int o, int m) {
@@ -348,7 +350,7 @@ int gain_upload(WarpJob *job, GainData *gd, int w, int h, const float *gain_map,
     job->gain_fy = gd->fy;
     job->gain_gw = gw;
     job->gain_gc = gc;
-    job->gain_mode = 1;
+    job->gain_mode = generic ? 3 : 1;
     return SB_OK;
 }
 }  // namespace sb

@@ -477,16 +477,31 @@ void resize_linear_taps(int n_src, int n_dst, bool columns, int *t)
 }
 
 // Taps of cv::resize(float32, INTER_LINEAR) as the reference's wheel computes it for the exposure compensator's gain
-// maps (IPP's kernel; found by hypothesis testing, see oracle/stitch_oracle.c): coordinate in double, fraction rounded
-// to float, zero where the index is clamped.
-void resize_f32_taps(int n_src, int n_dst, int *i0i1, float *fr)
+// maps (found by hypothesis testing, see oracle/stitch_oracle.c).  TAPS_IPP, a map with both sides >= 2 (IPP's kernel):
+// coordinate in double, fraction rounded to float, zero where the index is clamped.  TAPS_COLS / TAPS_ROWS, a map with a
+// side of 1 (OpenCV's own kernel): coordinate rounded to float, fraction in float; columns zero it where the index is
+// clamped, rows keep it and only clamp both indices.  A non-finite sample at a right-clamped column gives NaN where cv2
+// gives +-inf (it takes that sample alone); both round to the byte 0.
+void resize_f32_taps(int n_src, int n_dst, int *i0i1, float *fr, int form)
 {
-    const double scale = (double)n_src / (double)n_dst;
+    const double scale = (double)n_src / (double)n_dst, inv = 1.0 / ((double)n_dst / (double)n_src);
     for (int d = 0; d < n_dst; ++d) {
-        const double f = ((double)d + 0.5) * scale - 0.5;
-        const int s = (int)std::floor(f);
-        float t = (float)(f - (double)s);
-        if (s < 0 || s >= n_src - 1) t = 0.f;
+        int s;
+        float t;
+        if (form == TAPS_IPP) {
+            const double f = ((double)d + 0.5) * scale - 0.5;
+            s = (int)std::floor(f);
+            t = (float)(f - (double)s);
+            if (s < 0 || s >= n_src - 1) t = 0.f;
+        } else {
+            const float f = (float)(((double)d + 0.5) * inv - 0.5);
+            s = (int)std::floor(f);
+            t = f - (float)s;
+            if (form == TAPS_COLS && (s < 0 || s >= n_src - 1)) {
+                t = 0.f;
+                s = std::max(s, 0);  // the left end reads sample 0 and its neighbour (weights 1 and 0), as cv2 does
+            }
+        }
         i0i1[d] = std::min(std::max(s, 0), n_src - 1);
         i0i1[n_dst + d] = std::min(std::max(s + 1, 0), n_src - 1);
         fr[d] = t;

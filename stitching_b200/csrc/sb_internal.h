@@ -90,7 +90,8 @@ struct WarpJob {
     float xin_hi, yin_hi;  // 32 (sw-1) - 0.5, 32 (sh-1) - 0.5: upper limits of x*32, y*32 for a footprint inside the image
     // exposure compensation of the warped image (ExposureErrorCompensator.apply, stitcher.py:219-221), fused into the
     // warp's epilogue.  gain_mode 0: none; 1: float32 gain map (gain_gc = 1 or 3 channels) resized to dw x dh through
-    // the per-axis taps below (resize_f32_taps); 2: scalar gains as three 256-entry tables (gain_lut[c * 256 + value])
+    // the per-axis taps below (resize_f32_taps, TAPS_IPP); 2: scalar gains as three 256-entry tables
+    // (gain_lut[c * 256 + value]); 3: as 1 for a map with a side of 1 (TAPS_COLS / TAPS_ROWS, OpenCV's own passes)
     int gain_mode, gain_gw, gain_gc, gain_pad;
     const float *gain_map;
     const int *gain_tx, *gain_ty;    // [i0 | i1], dw / dh entries each
@@ -281,7 +282,8 @@ int launch_flush_l2(void *buf, size_t bytes, cudaStream_t s);
 int launch_wait_flags(const unsigned *flags, unsigned mask, unsigned value, cudaStream_t s);  // lanes with a mask bit wait for flags[lane] >= value
 // ExposureErrorCompensator.apply: taps of the float32 bilinear resize of a gain map (sb_geometry.cpp), the 256-entry
 // table of a scalar gain, and the host-buffer entry's kernel (sb_warp.cu)
-void resize_f32_taps(int n_src, int n_dst, int *i0i1, float *fr);  // i0i1: 2 * n_dst ints
+enum { TAPS_IPP = 0, TAPS_COLS = 1, TAPS_ROWS = 2 };  // resize_f32_taps' forms
+void resize_f32_taps(int n_src, int n_dst, int *i0i1, float *fr, int form);  // i0i1: 2 * n_dst ints
 void gain_scalar_lut(const double gain[3], uint8_t lut[768]);
 // rows copy; a fully contiguous image goes as ONE linear transfer (the DMA engines reach PCIe line rate with those)
 static inline cudaError_t sb_copy2d(void *dst, size_t dpitch, const void *src, size_t spitch, size_t width, size_t height,

@@ -53,8 +53,12 @@ __device__ __forceinline__ void project(const WarpJob &j, int u, int v, float &x
 
 // ExposureErrorCompensator.apply on one warped pixel (stitching/exposure_error_compensator.py:43-45 -> cv.detail
 // compensators, stitcher.py:219-221), see oracle/stitch_oracle.c for the pinned arithmetic:
-//   mode 1 (gain_blocks / channel_blocks): the float32 gain map resized to the warped size -- horizontal pass first, each
-//     pass a + (b - a) t as ONE fused multiply-add -- then saturate(cvRound(float(value) * gain)) with a float32 product;
+//   mode 1 (gain_blocks / channel_blocks, a map with both sides >= 2): the float32 gain map resized to the warped size as
+//     IPP's kernel does -- horizontal pass first, each pass a + (b - a) t as ONE fused multiply-add -- then
+//     saturate(cvRound(float(value) * gain)) with a float32 product;
+//   mode 3 (the same for a map with a side of 1, which cv::resize gives to OpenCV's own kernel): each pass
+//     a (1 - t) + b t as two rounded products and one rounded sum, 1 - t rounded too (fmul / fadd: nothing fuses, and the
+//     library is built -fmad=false), with the taps of TAPS_COLS / TAPS_ROWS;
 //   mode 2 (gain / channel): saturate(cvRound(double(value) * gain)), tabulated per channel on the host.
 __device__ __forceinline__ void apply_gain(const WarpJob &j, int u, int v, unsigned &r, unsigned &g, unsigned &b)
 {
@@ -66,6 +70,8 @@ __device__ __forceinline__ void apply_gain(const WarpJob &j, int u, int v, unsig
     }
     const int x0 = j.gain_tx[u], x1 = j.gain_tx[j.dw + u], y0 = j.gain_ty[v], y1 = j.gain_ty[j.dh + v];
     const float fx = j.gain_fx[u], fy = j.gain_fy[v];
+    const bool generic = j.gain_mode == 3;
+    const float ux = fadd(1.f, -fx), uy = fadd(1.f, -fy);
     const int gc = j.gain_gc;
     const float *r0 = j.gain_map + (long long)y0 * j.gain_gw * gc, *r1 = j.gain_map + (long long)y1 * j.gain_gw * gc;
     unsigned c[3] = {r, g, b};
@@ -74,8 +80,13 @@ __device__ __forceinline__ void apply_gain(const WarpJob &j, int u, int v, unsig
     for (int k = 0; k < 3; ++k) {
         if (k == 0 || gc == 3) {
             const float a0 = r0[x0 * gc + k], b0 = r0[x1 * gc + k], a1 = r1[x0 * gc + k], b1 = r1[x1 * gc + k];
-            const float h0 = fmaf(fadd(b0, -a0), fx, a0), h1 = fmaf(fadd(b1, -a1), fx, a1);
-            gain = fmaf(fadd(h1, -h0), fy, h0);
+            if (generic) {
+                const float h0 = fadd(fmul(a0, ux), fmul(b0, fx)), h1 = fadd(fmul(a1, ux), fmul(b1, fx));
+                gain = fadd(fmul(h0, uy), fmul(h1, fy));
+            } else {
+                const float h0 = fmaf(fadd(b0, -a0), fx, a0), h1 = fmaf(fadd(b1, -a1), fx, a1);
+                gain = fmaf(fadd(h1, -h0), fy, h0);
+            }
         }
         // cvRound(float) is cvtss2si: INT_MIN (so 0 after saturation) when the product leaves the int range or is NaN,
         // which set_gain's maps can make it; the device's saturating cvt would give 255

@@ -32,6 +32,7 @@ def corpora(L, O):
     import test_dropin_fuzz
     import test_final_scale
     import test_fullres
+    import test_gain_maps as GT
     import test_host_logic as H
     import test_shard_fuzz
     import test_timelapse_compositor as TL
@@ -70,11 +71,17 @@ def corpora(L, O):
                          ("blocks_tile_collapse", lambda mp: H.test_shared_memory_tile_kernels_under_block_emulation(L, O, mp)),
                          ("lanes_distance_transform", lambda mp: H.test_parallel_distance_transform_under_lane_emulation(L, O, mp))],
         "kernel_edges": [(cid, lambda mp, fn=fn: fn(O, mp)) for cid, fn in kernel_edges.emu_cases()],
+        "gain_maps": [(f"apply_{w}", lambda mp, w=w: GT.test_apply_against_the_compensators(L, O, w)) for w in ("1px", "ipp")]
+        + [("feed", lambda mp: GT.test_maps_fed_from_thin_low_images(L, O)),
+           ("device_twin", lambda mp: GT.test_device_twin_at_a_crop_offset(L, O)),
+           ("timelapse", lambda mp: GT.test_timelapse_with_clipped_parts(L, O)),
+           ("sharded", lambda mp: GT.test_sharded_owner_sets_the_gain(L, O))]
+        + [(f"compositor_{k}", lambda mp, k=k: GT.test_compositor_set_gain(L, O, k)) for k in (3, 4)],
     }
 
 
 NAMES = ["rig_fuzz", "crop_fuzz", "shard_fuzz", "dropin_fuzz", "final_scale", "timelapse_fuzz", "fullres", "goldens",
-         "setters", "lanes_blocks", "kernel_edges"]
+         "setters", "lanes_blocks", "kernel_edges", "gain_maps"]
 
 
 def run(lib_path, names, out=sys.stdout, only=None):

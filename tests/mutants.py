@@ -148,6 +148,32 @@ CATALOGUE = [
       "project(): a ray with z == 0 is divided (k_warp_wide's colour bytes of a zero-mask pixel change)", ["kernel_edges:z_zero_spherical", "kernel_edges:z_zero_cylindrical"], "index"),
     M("gain_cvt_sat", "sb_warp.cu", "const int q = cvt_rn_x86(fmul((float)c[k], gain));", "const int q = __float2int_rn(fmul((float)c[k], gain));",
       "apply_gain: a product outside the int range saturates to 255 instead of giving 0", ["goldens:gain_out_of_int_range", "kernel_edges:gain_2p31"], "rounding"),
+    # -- the gain map's resize (gain_upload's dispatch, resize_f32_taps, apply_gain's passes) ------------------------------
+    M("gain_ipp_unfused", "sb_warp.cu", "const float h0 = fmaf(fadd(b0, -a0), fx, a0), h1",
+      "const float h0 = fadd(fmul(fadd(b0, -a0), fx), a0), h1",
+      "apply_gain: the IPP tap of a map with both sides >= 2 rounded twice instead of fused", ["gain_maps:apply_ipp"], "rounding"),
+    M("gain_dispatch_and", "sb_api.cpp", "const bool generic = gw == 1 || gh == 1;", "const bool generic = gw == 1 && gh == 1;",
+      "gain_upload: a 1 x k or k x 1 map takes IPP's taps and passes (only 1 x 1 takes OpenCV's own)", ["gain_maps:timelapse"], "predicate"),
+    M("gain_rows_zeroed", "sb_geometry.cpp", "if (form == TAPS_COLS && (s < 0", "if (form != TAPS_IPP && (s < 0",
+      "resize_f32_taps: the rows of a map with a side of 1 zero the fraction at the clamped ends, as IPP does", ["gain_maps:compositor_3"],
+      "predicate"),
+    M("gain_coord_double", "sb_geometry.cpp",
+      "const float f = (float)(((double)d + 0.5) * inv - 0.5);\n            s = (int)std::floor(f);\n            t = f - (float)s;",
+      "const double f = ((double)d + 0.5) * inv - 0.5;\n            s = (int)std::floor(f);\n            t = (float)(f - (double)s);",
+      "resize_f32_taps: the coordinate of a map with a side of 1 kept in double instead of rounded to float", ["gain_maps:device_twin"],
+      "rounding"),
+    M("gain_cols_kept", "sb_geometry.cpp", "if (form == TAPS_COLS && (s < 0", "if (form == TAPS_IPP && (s < 0",
+      "resize_f32_taps: the columns of a map with a side of 1 keep the fraction at the clamped ends", ["gain_maps:apply_1px"], "predicate"),
+    M("gain_generic_fused", "sb_warp.cu", "const float h0 = fadd(fmul(a0, ux), fmul(b0, fx)), h1 = fadd(fmul(a1, ux), fmul(b1, fx));",
+      "const float h0 = fmaf(b0, fx, fmul(a0, ux)), h1 = fmaf(b1, fx, fmul(a1, ux));",
+      "apply_gain: the horizontal pass of a map with a side of 1 fused (a (1 - t) + b t with one rounding less)", ["gain_maps:apply_1px"],
+      "rounding"),
+    M("gain_generic_fused_rows", "sb_warp.cu", "gain = fadd(fmul(h0, uy), fmul(h1, fy));", "gain = fmaf(h1, fy, fmul(h0, uy));",
+      "apply_gain: the vertical pass of a map with a side of 1 fused", ["gain_maps:compositor_4"], "rounding"),
+    M("gain_ipp_float_coord", "sb_geometry.cpp", "const double f = ((double)d + 0.5) * scale - 0.5;\n            s = (int)std::floor(f);",
+      "const double f = (float)(((double)d + 0.5) * inv - 0.5);\n            s = (int)std::floor(f);",
+      "resize_f32_taps: the IPP fraction of a map with both sides >= 2 taken from the float-rounded coordinate", ["gain_maps:apply_ipp"],
+      "rounding"),
     M("resize_src_weights", "sb_warp.cu", "(unsigned)__ldg(j.tx + 2 * j.dw + x), (unsigned)__ldg(j.ty + 2 * dh + y));",
       "(unsigned)__ldg(j.ty + 2 * dh + y), (unsigned)__ldg(j.tx + 2 * j.dw + x));",
       "k_resize_src: the horizontal and vertical resize weights swapped", ["final_scale:kernel_0"], "operand"),
@@ -213,13 +239,14 @@ EQUIVALENT = [
     ("k_pyrdown_walk level >= 1: `BIN ? true : h_simd` -> `BIN ? false : h_simd` (and the same for v_simd)",
      "with binary masks the level-1 and level-2 weights are multiples of 2^-8 and 2^-16 whose partial sums stay below "
      "2^24 units (header of sb_pyrdown_fast.cu): every summation order is exact"),
+    ("resize_f32_taps, TAPS_IPP: the fraction zeroed only past the ends (`s >= n_src - 1` -> `s > n_src - 1`, and "
+     "`s < 0` -> `s < -1`)",
+     "at s == n_src - 1 (or s == -1) both indices clamp to the same sample, and fmaf(b - a, t, a) with b == a is a for "
+     "every t.  A non-finite sample gives NaN instead of +-inf there, and either rounds to the byte 0 in apply_gain"),
 ]
 
 # Candidates that are not equivalent but that no test of the suite kills yet: the next tests to write.
-OPEN = [
-    ("apply_gain: `fmaf(fadd(b0, -a0), fx, a0)` -> `fadd(fmul(..), a0)` (the gain-map tap rounded twice)",
-     "needs a gain map whose fused and unfused taps differ where value * gain sits at a rounding boundary"),
-]
+OPEN = []
 
 # -- device killers: run against a bound library on an H100 -----------------------------------------------------------------
 

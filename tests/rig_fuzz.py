@@ -571,6 +571,11 @@ def coverage(case, pyr_fast=True, tile=True, dt_fast=True, pd_bin=True):
         tags.add("feather w>8192")
         if dt_fast:
             tags.add("k_dt_rows_warp")
+    # gain_upload: a map with a side of 1 takes OpenCV's own resize taps (gain_mode 3), as cv::resize does
+    for _, _, g in extras(case):
+        if g is not None and g.dtype == np.float32 and 1 in g.shape[:2]:
+            gh, gw = g.shape[:2]
+            tags.add("gain map 1x1" if gh == gw else "gain map 1 px wide" if gw == 1 else "gain map 1 px high")
     return tags
 
 

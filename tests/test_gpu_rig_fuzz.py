@@ -36,7 +36,7 @@ def test_rig_fuzz_coverage_on_the_gpu(oracle):
         "tile l0 yes", "tile l0 no", "tile l1 yes", "nb=0", "nb=1", "nb>=2", "feather", "no", "blend width < 1", "n>32",
         "odd pano width", "z<=0", "map projection", "mixed extras", "feather w>8192", "k_dt_rows_warp",
         "k_warp_rgbm<HAS_BM=0>", "k_warp_rgbm<HAS_BM=1>", "k_warp_wide", "2-px source", "tile coarse 1 px wide",
-        "tile coarse 1 px high"}
+        "tile coarse 1 px high", "gain map 1 px wide", "gain map 1 px high", "gain map 1x1"}
     assert want <= reached, f"not reached: {sorted(want - reached)}"
     assert rig_fuzz.redraw_share(cs) < 0.5, f"{rig_fuzz.redraw_share(cs):.2f} rejected draws per case"
 

@@ -637,7 +637,7 @@ def test_rig_fuzz_coverage_under_emulation(oracle):
     want = {"nb=0", "nb=1", "nb>=2", "feather", "no", "n>32", "odd pano width", "map projection", "mixed extras",
             "gray blend mask", "k_warp_rgbm<HAS_BM=1>", "k_warp_rgbm<HAS_BM=0>", "tile l0 yes", "tile l0 no",
             "k_pyrdown_walk<1,0,1>", "k_pyrdown_walk<0,1,1>", "k_pyrdown_walk<0,0,0>", "k_pyrdown_walk<1,1,0>",
-            "tile coarse 1 px wide", "tile coarse 1 px high"}
+            "tile coarse 1 px wide", "tile coarse 1 px high", "gain map 1 px wide", "gain map 1 px high", "gain map 1x1"}
     assert want <= reached, f"not reached: {sorted(want - reached)}"
     lanes_gray = [c for c in cs if "SB_EMU_LANES" in c.env and c.blender == "multiband" and
                   any(m in ("ramp", "random") for m in c.masks)]
