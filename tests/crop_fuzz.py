@@ -7,15 +7,15 @@ rig_fuzz case scaled down by `aspect`, the LIR is drawn at random, and a duck-ty
 Crop.from_cropper -- so the draws reach slices clipped at the warped image's edge, placements that are not the warped
 corner plus the slice offset, and pano rois (hence band counts) that differ from the uncropped ones.
 
-SB_CROP_FUZZ_SEED=<int> replaces the fixed default seed.
+SB_CROP_FUZZ_SEED=<int> or =random replaces the fixed default seed (the seed used is printed).
 """
 import dataclasses
-import math
-import os
+import functools
 import types
 
 import numpy as np
 
+import fuzz_chain
 import rig_fuzz
 from stitching_b200 import Compositor, Crop
 
@@ -23,9 +23,7 @@ DEFAULT_SEED = 20261016
 ASPECTS = (1.0, 1.5, 2.5, 0.5, 1.25, 3.0, 1.7)  # x.5 and x.25 products round half to even
 
 
-def seed_from_env():
-    s = os.environ.get("SB_CROP_FUZZ_SEED")
-    return int(s) if s else DEFAULT_SEED
+seed_from_env = functools.partial(fuzz_chain.seed_from_env, "SB_CROP_FUZZ_SEED", DEFAULT_SEED)
 
 
 def _overlap(r, lir):
@@ -62,6 +60,7 @@ class CropCase:
     case: object      # rig_fuzz.Case (rects: the uncropped warped rects)
     crop: object      # Crop
     aspect: float
+    low: object = None  # the LOW Cropper it was drawn as (fuzz_chain.draw_crop)
 
     @property
     def n(self):
@@ -90,17 +89,9 @@ def cases(seed, count, budget):
     for c in rig_fuzz.cases(seed, 4 * count, budget):
         if len(out) == count:
             break
-        for _ in range(20):
-            aspect = float(rng.choice(ASPECTS))
-            frac = (rng.uniform(0, 0.3), rng.uniform(0, 0.3), rng.uniform(0.7, 1.0), rng.uniform(0.7, 1.0))
-            cr = low_cropper(c.rects, aspect, frac)
-            if cr is None:
-                continue
-            crop = Crop.from_cropper(cr, aspect)
-            cc = CropCase(c, crop, aspect)
-            if all(w > 0 and h > 0 for _, _, w, h in cc.fed()):
-                out.append(cc)
-                break
+        cc = fuzz_chain.draw_crop(rng, c, ASPECTS, 0.3, 0.7)
+        if cc is not None:
+            out.append(cc)
     return out
 
 
@@ -115,65 +106,28 @@ def named(name, budget):
 
 
 # -- the two sides ----------------------------------------------------------------------------------------------------
-def oracle_run(O, cc, imgs, ex, s16=False):
-    """Stitcher order: warp, slice image and mask (a numpy slice), compensator apply on the cropped image, blend mask =
-    the caller's mask or SeamFinder.resize(seam, cropped mask) or the cropped mask; Blender.prepare(cropped corners,
-    sizes), feed at the cropped corners, blend.  `raw` and "pano16" as in rig_fuzz.oracle_run."""
-    case = cc.case
-    scale = case.scale()
-    warped, masks, raw = [], [], []
-    for img, cam, (x, y, w, h), (mask, seam, gain) in zip(imgs, case.cams, cc.crop.rects, ex):
-        _, wi, wm = O.warp(case.wtype, scale, rig_fuzz.Warper.get_K(cam, 1), cam.R, img)
-        raw.append((wi, wm))
-        wi = np.ascontiguousarray(wi[y:y + h, x:x + w])
-        wm = np.ascontiguousarray(wm[y:y + h, x:x + w])
-        if gain is not None:
-            wi = O.gain_apply(wi, gain)
-        if mask is not None:
-            wm = mask
-        elif seam is not None:
-            wm = O.seam_resize(seam, wm)
-        warped.append(wi)
-        masks.append(wm)
-    b = O.Blender(case.blender, case.strength)
-    b.prepare(cc.crop.corners, cc.crop.sizes)
-    for wi, wm, c in zip(warped, masks, cc.crop.corners):
-        b.feed(wi, wm, c)
-    pano16, pmask = b.blend_s16()
-    rects = [tuple(c) + (wi.shape[1], wi.shape[0]) for c, wi in zip(cc.crop.corners, warped)]
-    return dict(warped=warped, masks=masks, rects=rects, roi=b.roi, num_bands=b.num_bands if b._kind == "multiband" else -1,
-                pano=O.convert_scale_abs(pano16), pmask=pmask, raw=raw, pano16=pano16 if s16 else None)
-
-
 def compositor(cc, crop=True, **kw):
     case = cc.case
     return Compositor(case.cams, case.sizes, case.wtype, case.blender, case.strength, crop=cc.crop if crop else None, **kw)
 
 
-def compositor_run(cc, imgs, ex):
-    c = compositor(cc)
-    try:
-        for i, (mask, seam, gain) in enumerate(ex):
-            if mask is not None:
-                c.set_mask(i, mask)
-            if seam is not None:
-                c.set_seam_mask(i, seam)
-            if gain is not None:
-                c.set_gain(i, gain)
-        pano, pmask = c.composite(imgs)
-        warped = [c.download_warped(i) for i in range(cc.n)]
-        return dict(rects=list(c.rects), roi=tuple(c.roi), num_bands=c.num_bands, pano=pano, pmask=pmask,
-                    warped=[w for w, _ in warped], masks=[m for _, m in warped])
-    finally:
-        c.close()
-
-
 def run_and_check(O, cc, seed):
     imgs, ex = rig_fuzz.images(cc.case), rig_fuzz.extras(cc.cropped_case())
-    ref = oracle_run(O, cc, imgs, ex)
-    got = compositor_run(cc, imgs, ex)
+    ref = rig_fuzz.oracle_run(O, cc.case, imgs, ex, crop=cc.crop)
+    got = fuzz_chain.compositor_run(cc.case, imgs, ex, crop=cc.crop)
     rig_fuzz.check(dataclasses.replace(cc.case, name=cc.describe()), got, ref, seed)
     return got
+
+
+def ab_arrays(seed, count, ks):
+    """Cases `ks` of cases(seed, count, GPU) through the compositor: the pano and its mask by name."""
+    cs = cases(seed, count, rig_fuzz.GPU)
+    out = {}
+    for k in ks:
+        got = fuzz_chain.compositor_run(cs[k].case, rig_fuzz.images(cs[k].case), rig_fuzz.extras(cs[k].cropped_case()),
+                                        crop=cs[k].crop)
+        out[f"{k}_pano"], out[f"{k}_pmask"] = got["pano"], got["pmask"]
+    return out
 
 
 # -- sharded ------------------------------------------------------------------------------------------------------------
@@ -182,100 +136,56 @@ def sharded_cases(seed, count, budget):
     grouped oracle prepares from the fed images)."""
     import shard_fuzz
 
+    def keep(cc):
+        g = fuzz_chain.blend_geometry(cc.crop.corners, cc.crop.sizes, cc.case.blender, cc.case.strength)
+        blends = g.nb >= 1 if g.kind == "multiband" else g.kind == "feather"
+        return blends and g.roi == fuzz_chain.blend_geometry(cc.crop.corners, [f[2:] for f in cc.fed()]).roi
+
     rng = np.random.default_rng(seed)
     out = []
     for c in shard_fuzz.cases(seed, 4 * count, budget):
         if len(out) == count:
             break
-        for _ in range(20):
-            aspect = float(rng.choice(ASPECTS))
-            frac = (rng.uniform(0, 0.2), rng.uniform(0, 0.2), rng.uniform(0.8, 1.0), rng.uniform(0.8, 1.0))
-            cr = low_cropper(c.rects, aspect, frac)
-            if cr is None:
-                continue
-            cc = CropCase(c, Crop.from_cropper(cr, aspect), aspect)
-            fed = cc.fed()
-            _, _, w, h = _roi(cc.crop.corners, cc.crop.sizes)
-            blends = _bands(c, w, h) >= 1 if c.blender == "multiband" else math.sqrt(w * h) * c.strength >= 100.0
-            if blends and all(f[2] > 0 and f[3] > 0 for f in fed) and \
-                    _roi(cc.crop.corners, cc.crop.sizes) == _roi(cc.crop.corners, [f[2:] for f in fed]):
-                out.append(cc)
-                break
+        cc = fuzz_chain.draw_crop(rng, c, ASPECTS, 0.2, 0.8, keep=keep)
+        if cc is not None:
+            out.append(cc)
     return out
 
 
 def sharded_check(O, cc, world, copy, seed):
-    """All ranks in this process through the transport hooks: every rank's own cropped warped images and its strip equal
-    shard_fuzz.grouped_blend fed with the cropped images.  Returns False when the crop's blocks run right to left (the
-    sharded composite refuses those)."""
+    """All ranks in this process through the transport hooks (shard_fuzz.hooks_run with the crop): every rank's own
+    cropped warped images and its strip equal shard_fuzz.grouped_blend fed with the cropped images.  Returns False
+    when the crop's blocks run right to left (the sharded composite refuses those)."""
     import replay
     import shard_fuzz
     from stitching_b200 import StitchingError
 
-    case = cc.case
+    case = dataclasses.replace(cc.case, world=world)
     imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(cc.cropped_case())
-    ref = oracle_run(O, cc, imgs, ex)
+    ref = rig_fuzz.oracle_run(O, case, imgs, ex, crop=cc.crop)
     _, panos = shard_fuzz.grouped_blend(O, case.blender, case.strength, cc.crop.corners, ref["warped"], ref["masks"], world)
-    ranks = []
     try:
-        try:
-            for r in range(world):
-                ranks.append(compositor(cc, rank=r, world=world))
-        except StitchingError as e:
-            if "right to left" in str(e) or "order" in str(e):
-                return False
-            raise
-        for c in ranks:
-            for i in range(c.first, c.first + c.count):
-                mask, seam, gain = ex[i]
-                if mask is not None:
-                    c.set_mask(i, mask)
-                if seam is not None:
-                    c.set_seam_mask(i, seam)
-                if gain is not None:
-                    c.set_gain(i, gain)
-            c.upload(imgs[c.first: c.first + c.count])
-            c.shard_phase(0)
-        for src in ranks:
-            for dst in ranks:
-                if src is not dst:
-                    sp, sn = src.shard_slab(dst.rank, True)
-                    dp, dn = dst.shard_slab(src.rank, False)
-                    assert sn == dn
-                    if sn:
-                        copy(dp, sp, sn)
-        where = f"seed {seed}, {cc.describe()}, world {world}"
-        for c in ranks:
-            c.shard_phase(1)
-            assert [tuple(x) for x in c.rects] == ref["rects"] and tuple(c.roi) == tuple(ref["roi"]), where
-            assert c.num_bands == ref["num_bands"], where
-            for i in range(c.first, c.first + c.count):
-                wi, wm = c.download_warped(i)
-                replay.assert_exact(wi, ref["warped"][i], f"{where}: warped image {i}")
-                replay.assert_exact(wm, ref["masks"][i], f"{where}: warped mask {i}")
-            pano, pmask = c.download()
-            rp, rm = panos[c.rank]
-            replay.assert_exact(pano, shard_fuzz.cut(rp, c.strip, c.strip_axis), f"{where}: rank {c.rank} strip")
-            replay.assert_exact(pmask, shard_fuzz.cut(rm, c.strip, c.strip_axis), f"{where}: rank {c.rank} strip mask")
-        return True
-    finally:
-        for c in ranks:
-            c.close()
+        got, slabs = shard_fuzz.hooks_run(case, imgs, ex, copy, crop=cc.crop)
+    except StitchingError as e:
+        if "right to left" in str(e) or "order" in str(e):
+            return False
+        raise
+    where = f"seed {seed}, {cc.describe()}, world {world}"
+    for sn, dn in slabs.values():
+        assert sn == dn, where
+    for r, rk in enumerate(got):
+        assert [tuple(x) for x in rk["rects"]] == ref["rects"] and tuple(rk["roi"]) == tuple(ref["roi"]), where
+        assert rk["num_bands"] == ref["num_bands"], where
+        for i, (wi, wm) in rk["warped"].items():
+            replay.assert_exact(wi, ref["warped"][i], f"{where}: warped image {i}")
+            replay.assert_exact(wm, ref["masks"][i], f"{where}: warped mask {i}")
+        rp, rm = panos[r]
+        replay.assert_exact(rk["pano"], shard_fuzz.cut(rp, rk["strip"], rk["axis"]), f"{where}: rank {r} strip")
+        replay.assert_exact(rk["pmask"], shard_fuzz.cut(rm, rk["strip"], rk["axis"]), f"{where}: rank {r} strip mask")
+    return True
 
 
 # -- coverage -----------------------------------------------------------------------------------------------------------
-def _roi(corners, sizes):
-    x0, y0 = min(c[0] for c in corners), min(c[1] for c in corners)
-    return x0, y0, max(c[0] + s[0] for c, s in zip(corners, sizes)) - x0, max(c[1] + s[1] for c, s in zip(corners, sizes)) - y0
-
-
-def _bands(case, w, h):
-    bw = math.sqrt(w * h) * case.strength / 100.0
-    if case.blender != "multiband" or bw < 1.0:
-        return -1
-    return min(int(math.log(bw) / math.log(2.0) - 1.0), int(math.ceil(math.log(max(w, h)) / math.log(2.0))))
-
-
 def coverage(cc):
     """What a crop case reaches, from its geometry alone."""
     case = cc.case
@@ -284,14 +194,15 @@ def coverage(cc):
         tags.add("map projection")
     if case.n > rig_fuzz.WARP_BATCH:
         tags.add("n>32")
-    _, _, w, h = _roi(cc.crop.corners, cc.crop.sizes)
-    nb = _bands(case, w, h)
+    g = fuzz_chain.blend_geometry(cc.crop.corners, cc.crop.sizes, case.blender, case.strength)
+    _, _, w, h = g.roi
+    nb = g.nb if g.kind == "multiband" else -1
     if nb >= 0:
         tags.add("nb=0" if nb == 0 else "nb=1" if nb == 1 else "nb>=2")
         if nb >= 1:
             tags.add("tile l0 yes" if w % 2 == 0 else "tile l0 no")
-    x, y, W, H = case.roi()
-    if nb != _bands(case, W, H):
+    whole = case.geometry()
+    if nb != (whole.nb if whole.kind == "multiband" else -1):
         tags.add("crop changes num_bands")
     fed = cc.fed()
     if any((f[2], f[3]) != tuple(s) for f, s in zip(fed, cc.crop.sizes)):

@@ -5,8 +5,8 @@ The drop-ins are what install() puts under every reference Stitcher, so they run
 (cropper.py:150-151); ExposureErrorCompensator.apply with a compensator whose getMatGains() hands out the case's gains;
 SeamFinder.resize (with cv.UMat seam masks for a share of the cases, as the seam finders hand them out); Blender prepare /
 feed / blend, with the int16 result for a share of the multiband cases; and, for some cases, the Timelapser over the same
-images.  The oracle side is rig_fuzz.oracle_run / crop_fuzz.oracle_run on the same draws; everything is compared bit
-for bit.
+images.  The oracle side is rig_fuzz.oracle_run on the same draws, with the crop where there is one; everything is
+compared bit for bit.
 
 Every case also picks, per image, how the image travels from the warp to the blender (FEEDS):
   twin  the warped image's device twin throughout: sb_gain_apply_dev, sb_blender_feed_dev (k_pack_rgbm from the twin's
@@ -20,15 +20,16 @@ seed), and drop-in-only draws: 1-px source sides, source widths of every residue
 paired loads), sources passed as column-sliced views (row pitch > 3 w), strengths that are not float32-exact and
 timelapse frames.
 
-SB_DROPIN_FUZZ_SEED=<int> replaces the fixed default seed of the drop-in choices and draws.
+SB_DROPIN_FUZZ_SEED=<int> or =random replaces the fixed default seed of the drop-in choices and draws (the seed used
+is printed).
 """
 import dataclasses
-import math
-import os
+import functools
 
 import numpy as np
 
 import crop_fuzz
+import fuzz_chain
 import rig_fuzz
 
 DEFAULT_SEED = 20261017
@@ -36,9 +37,7 @@ FEEDS = ("twin", "host", "s16")
 LANES, BLOCKS = rig_fuzz.LANES, rig_fuzz.BLOCKS
 
 
-def seed_from_env():
-    s = os.environ.get("SB_DROPIN_FUZZ_SEED")
-    return int(s) if s else DEFAULT_SEED
+seed_from_env = functools.partial(fuzz_chain.seed_from_env, "SB_DROPIN_FUZZ_SEED", DEFAULT_SEED)
 
 
 @dataclasses.dataclass
@@ -171,15 +170,7 @@ def own_cases(seed, count, budget, env_every=0):
         c.redraws = redraws
         s = rig_fuzz._strength(rng, c.rects, c.blender)
         c.strength = _inexact(rng, s) if rng.random() < 0.85 else s
-        cc = None
-        if rng.random() < 0.4:
-            aspect = float(rng.choice(crop_fuzz.ASPECTS))
-            frac = (rng.uniform(0, 0.3), rng.uniform(0, 0.3), rng.uniform(0.7, 1.0), rng.uniform(0.7, 1.0))
-            cr = crop_fuzz.low_cropper(c.rects, aspect, frac)
-            if cr is not None:
-                cc = crop_fuzz.CropCase(c, crop_fuzz.Crop.from_cropper(cr, aspect), aspect)
-                if not all(w > 0 and h > 0 for _, _, w, h in cc.fed()):
-                    cc = None
+        cc = fuzz_chain.draw_crop(rng, c, crop_fuzz.ASPECTS, 0.3, 0.7, tries=1) if rng.random() < 0.4 else None
         dc = _choose(rng, c.name, c, cc)
         dc.views = bool(rng.random() < 0.5)
         if c.n <= 6 and rng.random() < 0.35:
@@ -254,8 +245,7 @@ class GainCompensator:
 
 # -- the two sides ------------------------------------------------------------------------------------------------------
 def oracle_run(O, dc, imgs, ex):
-    ref = (crop_fuzz.oracle_run(O, dc.crop, imgs, ex, s16=dc.s16_out) if dc.crop is not None else
-           rig_fuzz.oracle_run(O, dc.case, imgs, ex, s16=dc.s16_out))
+    ref = rig_fuzz.oracle_run(O, dc.case, imgs, ex, s16=dc.s16_out, crop=dc.crop.crop if dc.crop is not None else None)
     if dc.timelapse:
         corners, sizes = dc.corners_sizes()
         t = O.Timelapser(dc.timelapse)
@@ -370,15 +360,8 @@ def run_and_check(O, dc, seed):
 def plan(dc):
     """(blend kind, band count, pano width) of Blender.prepare on the prepared corners and sizes, in double like the
     reference; band count -1 when not multiband."""
-    corners, sizes = dc.corners_sizes()
-    _, _, w, h = crop_fuzz._roi(corners, sizes)
-    bw = math.sqrt(w * h) * dc.case.strength / 100.0
-    if dc.case.blender == "no" or bw < 1.0:
-        return "no", -1, w
-    if dc.case.blender == "feather":
-        return "feather", -1, w
-    nb = int(math.log(bw) / math.log(2.0) - 1.0)
-    return "multiband", min(nb, int(math.ceil(math.log(max(w, h)) / math.log(2.0)))), w
+    g = fuzz_chain.blend_geometry(*dc.corners_sizes(), dc.case.blender, dc.case.strength)
+    return g.kind, g.nb if g.kind == "multiband" else -1, g.roi[2]
 
 
 def footprints(O, dc, i):

@@ -16,14 +16,15 @@ Records.  tests/golden/gen_final_scale_golden.py ran the unmodified reference St
 exactly) and 5 on the 4 views of 4000 x 3000 of golden_fullres_a; the records hold the fullres fields plus "resized",
 the digest of every frame resize_final_resolution handed to the warp.
 
-SB_FINAL_SCALE_SEED=<int> replaces the fixed default seed.
+SB_FINAL_SCALE_SEED=<int> or =random replaces the fixed default seed (the seed used is printed).
 """
 import dataclasses
-import os
+import functools
 
 import numpy as np
 
 import fullres
+import fuzz_chain
 import reference_cases as RC
 import replay
 import rig_fuzz
@@ -33,9 +34,7 @@ DEFAULT_SEED = 20261019
 RECORDS = ("3", "5")
 
 
-def seed_from_env():
-    s = os.environ.get("SB_FINAL_SCALE_SEED")
-    return int(s) if s else DEFAULT_SEED
+seed_from_env = functools.partial(fuzz_chain.seed_from_env, "SB_FINAL_SCALE_SEED", DEFAULT_SEED)
 
 
 # -- kernel draws -------------------------------------------------------------------------------------------------------
@@ -118,33 +117,14 @@ def oracle_resized(O, imgs, sizes):
     return [img if (img.shape[1], img.shape[0]) == tuple(s) else O.resize_linear_exact(img, s) for img, s in zip(imgs, sizes)]
 
 
-def compositor_run(case, imgs, ex, crop=None, **kw):
-    """rig_fuzz.compositor_run with a crop and Compositor keywords (input_sizes)."""
-    c = Compositor(case.cams, case.sizes, case.wtype, case.blender, case.strength, crop=crop, **kw)
-    try:
-        for i, (mask, seam, gain) in enumerate(ex):
-            if mask is not None:
-                c.set_mask(i, mask)
-            if seam is not None:
-                c.set_seam_mask(i, seam)
-            if gain is not None:
-                c.set_gain(i, gain)
-        pano, pmask = c.composite(imgs)
-        warped = [c.download_warped(i) for i in range(case.n)]
-        return dict(rects=list(c.rects), roi=tuple(c.roi), num_bands=c.num_bands, pano=pano, pmask=pmask,
-                    warped=[w for w, _ in warped], masks=[m for _, m in warped])
-    finally:
-        c.close()
-
-
 def rig_check(O, case, seed, crop=None, ex=None):
     """The compositor fed camera frames equals the compositor fed the oracle's resize of them, byte for byte."""
     rng = np.random.default_rng([seed, case.seed])
     ins = input_sizes(case, rng)
     cams = frames(ins, case.seed)
     ex = rig_fuzz.extras(case) if ex is None else ex
-    want = compositor_run(case, oracle_resized(O, cams, case.sizes), ex, crop)
-    got = compositor_run(case, cams, ex, crop, input_sizes=ins)
+    want = fuzz_chain.compositor_run(case, oracle_resized(O, cams, case.sizes), ex, crop=crop)
+    got = fuzz_chain.compositor_run(case, cams, ex, crop=crop, input_sizes=ins)
     rig_fuzz.check(dataclasses.replace(case, name=f"{case.describe()} inputs {ins}"), got, want, seed)
     return ins
 
@@ -152,8 +132,6 @@ def rig_check(O, case, seed, crop=None, ex=None):
 def sharded_check(O, case, world, copy, seed):
     """All ranks through the transport hooks, fed camera frames: equal to shard_fuzz's grouped oracle fed the
     oracle's resized frames."""
-    import functools
-
     import shard_fuzz
 
     case = dataclasses.replace(case, world=world)
@@ -162,7 +140,7 @@ def sharded_check(O, case, world, copy, seed):
     cams = frames(ins, case.seed)
     ex = [(None, None, None)] * case.n
     ref = shard_fuzz.grouped_oracle(O, case, oracle_resized(O, cams, case.sizes), ex, world)
-    got, slabs = shard_fuzz.hooks_run(functools.partial(Compositor, input_sizes=ins), case, cams, ex, copy)
+    got, slabs = shard_fuzz.hooks_run(case, cams, ex, copy, input_sizes=ins)
     shard_fuzz.check(case, got, slabs, ref, seed)
 
 
@@ -230,6 +208,18 @@ def compositor(z, crop=True, **kw):
         c.set_seam_mask(i, fullres.seams(z)[i])
         c.set_gain(i, fullres.gains(z)[i])
     return c
+
+
+def ab_arrays(name):
+    """Record `name` through the compositor from its camera views: the pano, its mask and every warped image and mask."""
+    z = record(name)
+    c = compositor(z)
+    try:
+        pano, mask = c.composite(views(z))
+        return dict(pano=pano, mask=mask, warped=np.concatenate([np.concatenate([a.ravel(), b.ravel()])
+                                                                 for a, b in (c.download_warped(i) for i in range(c.n))]))
+    finally:
+        c.close()
 
 
 def compositor_replay(z, views):

@@ -12,19 +12,20 @@ compositor, the drop-in classes or the oracle and a mismatch names its stage.
 Ratio draws.  Crops of rig_fuzz-style rigs at FINAL sizes of 1500-4000 px seen from a LOW resolution at the ratios the
 Stitcher's own formula gives for 2-48 MP cameras, sqrt(MP / 0.1), with LOW seam masks and 32 px block gain maps sized
 from the LOW cropped images, as the seam finder and the gain_blocks compensator hand them out.  They go through the
-compositor against crop_fuzz's oracle order of operations; coverage() restates from the geometry what each reaches.
+compositor against rig_fuzz.oracle_run with the crop; coverage() restates from the geometry what each reaches.
 
-SB_FULLRES_SEED=<int> replaces the fixed default seed of the ratio draws.
+SB_FULLRES_SEED=<int> or =random replaces the fixed default seed of the ratio draws (the seed used is printed).
 """
 import dataclasses
+import functools
 import math
-import os
 import time
 import types
 
 import numpy as np
 
 import crop_fuzz
+import fuzz_chain
 import reference_cases as RC
 import replay
 import rig_fuzz
@@ -36,9 +37,7 @@ DEFAULT_SEED = 20261018
 BLOCK = 32   # the gain_blocks compensator's block size at LOW resolution (ExposureErrorCompensator.DEFAULT_BLOCK_SIZE)
 
 
-def seed_from_env():
-    s = os.environ.get("SB_FULLRES_SEED")
-    return int(s) if s else DEFAULT_SEED
+seed_from_env = functools.partial(fuzz_chain.seed_from_env, "SB_FULLRES_SEED", DEFAULT_SEED)
 
 
 # -- the records --------------------------------------------------------------------------------------------------------
@@ -131,8 +130,8 @@ def diff_table(got, ref, what):
 
 
 class OracleChain:
-    """The FINAL chain of a record on the CPU oracle, image by image, built only when a stage has to be explained (or
-    pinned): warp, numpy slice, gain_apply, seam_resize; the blend only for the panorama."""
+    """The FINAL chain of a record on the CPU oracle (fuzz_chain.oracle_image), image by image, built only when a stage
+    has to be explained (or pinned); the blend only for the panorama."""
 
     def __init__(self, O, z, imgs):
         self.O, self.z, self.imgs = O, z, imgs
@@ -145,12 +144,12 @@ class OracleChain:
             from stitching_b200.warper import Warper
 
             cam, (x, y, w, h) = self.cams[i], self.crop.rects[i]
-            _, wi, wm = self.O.warp("spherical", self.scale, Warper.get_K(cam, self.z["medium_to_final"]), cam.R, self.imgs[i])
-            ci, cm = np.ascontiguousarray(wi[y:y + h, x:x + w]), np.ascontiguousarray(wm[y:y + h, x:x + w])
-            comp = self.O.gain_apply(ci, gains(self.z)[i])
+            (_, wi, wm), comp, bm = fuzz_chain.oracle_image(self.O, "spherical", self.scale,
+                                                            Warper.get_K(cam, self.z["medium_to_final"]), cam.R, self.imgs[i],
+                                                            (x, y, w, h), gains(self.z)[i], seam=seams(self.z)[i])
             # one image at a time: the stages of a 48 MP image take over half a GB
-            self._cache = {i: dict(warped=wi, warped_mask=wm, cropped=ci, cropped_mask=cm, compensated=comp,
-                                   blend_mask=self.O.seam_resize(seams(self.z)[i], cm))}
+            self._cache = {i: dict(warped=wi, warped_mask=wm, cropped=wi[y:y + h, x:x + w], cropped_mask=wm[y:y + h, x:x + w],
+                                   compensated=comp, blend_mask=bm)}
         return self._cache[i]
 
     def stage(self, stage, i):
@@ -188,9 +187,7 @@ def compositor_replay(z, imgs, oracle=None):
     try:
         n = int(z["n"])
         assert [tuple(r) for r in c.rects] == fed_rects(z), f"rects {c.rects} != {fed_rects(z)}"
-        corners, sizes = [tuple(map(int, v)) for v in z["corners"]], [tuple(map(int, v)) for v in z["sizes"]]
-        x0, y0 = min(x for x, _ in corners), min(y for _, y in corners)
-        roi = (x0, y0, max(x + w for (x, _), (w, _) in zip(corners, sizes)) - x0, max(y + h for (_, y), (_, h) in zip(corners, sizes)) - y0)
+        roi = fuzz_chain.blend_geometry([tuple(map(int, v)) for v in z["corners"]], [tuple(map(int, v)) for v in z["sizes"]]).roi
         assert tuple(c.roi) == roi, f"pano roi {c.roi} != {roi}"
         assert c.num_bands == int(z["num_bands"]), f"num_bands {c.num_bands} != {int(z['num_bands'])}"
         pano, pmask = c.composite(imgs)
@@ -307,17 +304,9 @@ def cases(seed, count, lo, hi, max_area):
         if c.blender == "multiband" and rng.random() < 0.5:
             c.strength = rig_fuzz._strength(rng, c.rects, c.blender)
         mp = float(rng.choice([2, 5, 8, 12, 16, 20, 24, 33, 48])) * float(rng.uniform(0.97, 1.03))
-        aspect = pipeline_aspect(mp)
-        for _ in range(20):
-            frac = (rng.uniform(0, 0.3), rng.uniform(0, 0.3), rng.uniform(0.7, 1.0), rng.uniform(0.7, 1.0))
-            cr = crop_fuzz.low_cropper(c.rects, aspect, frac)
-            if cr is None:
-                continue
-            cc = crop_fuzz.CropCase(c, Crop.from_cropper(cr, aspect), aspect)
-            if all(w > 0 and h > 0 for _, _, w, h in cc.fed()):
-                cc.low = cr
-                out.append(cc)
-                break
+        cc = fuzz_chain.draw_crop(rng, c, pipeline_aspect(mp), 0.3, 0.7)
+        if cc is not None:
+            out.append(cc)
     return out
 
 
@@ -342,8 +331,8 @@ def extras(cc):
 
 def run_and_check(O, cc, seed):
     imgs, ex = rig_fuzz.images(cc.case), extras(cc)
-    ref = crop_fuzz.oracle_run(O, cc, imgs, ex)
-    got = crop_fuzz.compositor_run(cc, imgs, ex)
+    ref = rig_fuzz.oracle_run(O, cc.case, imgs, ex, crop=cc.crop)
+    got = fuzz_chain.compositor_run(cc.case, imgs, ex, crop=cc.crop)
     rig_fuzz.check(dataclasses.replace(cc.case, name=cc.describe()), got, ref, seed)
     return sum(a.size for a in got["warped"] + got["masks"]) + got["pano"].size + got["pmask"].size
 

@@ -333,7 +333,7 @@ def check_sharded(O, copy, scale_down=16):
     maps = probe_maps(13) + [np.random.default_rng(5).uniform(0.6, 1.5, (3, 4)).astype(np.float32)]
     ex = [(None, None, maps[i % len(maps)]) for i in range(case.n)]
     ref = shard_fuzz.grouped_oracle(O, case, imgs, ex)
-    got, sizes = shard_fuzz.hooks_run(Compositor, case, imgs, ex, copy)
+    got, sizes = shard_fuzz.hooks_run(case, imgs, ex, copy)
     shard_fuzz.check(case, got, sizes, ref, 0)
 
 

@@ -210,12 +210,12 @@ def bin_case(seed):
 
 
 def check_bin(O, seed):
+    import fuzz_chain
     import rig_fuzz
-    from stitching_b200 import Compositor
 
     c = bin_case(seed)
     imgs, ex = rig_fuzz.images(c), rig_fuzz.extras(c)
-    rig_fuzz.check(c, rig_fuzz.compositor_run(Compositor, c, imgs, ex), rig_fuzz.oracle_run(O, c, imgs, ex), seed)
+    rig_fuzz.check(c, fuzz_chain.compositor_run(c, imgs, ex), rig_fuzz.oracle_run(O, c, imgs, ex), seed)
 
 
 # -- the case lists ------------------------------------------------------------------------------------------------------

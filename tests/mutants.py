@@ -253,16 +253,16 @@ OPEN = []
 
 def _gpu_rig_fuzz_compositor(L):
     """The GPU rig set's multiband cases with at least four bands (binary and gray masks), bit for bit."""
+    import fuzz_chain
     import rig_fuzz
     from oracle import oracle as O
-    from stitching_b200 import Compositor
-
+    
     O.build()
     cs = rig_fuzz.gpu_set(rig_fuzz.DEFAULT_SEED)
     picked = [c for c in cs if rig_fuzz.plan(c)[0] == "multiband" and rig_fuzz.plan(c)[1] >= 4][:12]
     for c in picked:
         imgs, ex = rig_fuzz.images(c), rig_fuzz.extras(c)
-        rig_fuzz.check(c, rig_fuzz.compositor_run(Compositor, c, imgs, ex), rig_fuzz.oracle_run(O, c, imgs, ex), rig_fuzz.DEFAULT_SEED)
+        rig_fuzz.check(c, fuzz_chain.compositor_run(c, imgs, ex), rig_fuzz.oracle_run(O, c, imgs, ex), rig_fuzz.DEFAULT_SEED)
 
 
 def _gpu_edges(L):
@@ -275,14 +275,14 @@ def _gpu_edges(L):
 
 
 def _gpu_wide_feather(L):
+    import fuzz_chain
     import rig_fuzz
     from oracle import oracle as O
-    from stitching_b200 import Compositor
-
+    
     O.build()
     c = rig_fuzz.named("wide_feather", rig_fuzz.GPU)
     imgs, ex = rig_fuzz.images(c), rig_fuzz.extras(c)
-    rig_fuzz.check(c, rig_fuzz.compositor_run(Compositor, c, imgs, ex), rig_fuzz.oracle_run(O, c, imgs, ex), 0)
+    rig_fuzz.check(c, fuzz_chain.compositor_run(c, imgs, ex), rig_fuzz.oracle_run(O, c, imgs, ex), 0)
 
 
 def _gpu_division(L):

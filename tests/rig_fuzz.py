@@ -14,12 +14,13 @@ that a test can prove which branches a seeded set of cases reached.
 SB_RIG_FUZZ_SEED=<int> or =random replaces the fixed default seed (the seed used is printed).
 """
 import dataclasses
+import functools
 import math
-import os
 from statistics import median
 
 import numpy as np
 
+import fuzz_chain
 from stitching_b200 import rigs
 from stitching_b200.warper import Warper
 
@@ -28,18 +29,12 @@ EMU = dict(side=120, area=14_000)         # emulation build: serial CPU stand-in
 GPU = dict(side=1500, area=1_200_000)     # H100: the oracle (scalar C on the CPU) sets the cost
 TABLE_TYPES = ("spherical", "cylindrical", "plane", "affine", "mercator")  # k_warp_rgbm from separable tables
 MAP_TYPES = ("fisheye", "stereographic")                                 # host-built maps, k_warp_wide writes RGBM
-WARP_BATCH = 32        # SB_WARP_BATCH (sb_internal.h:210)
+WARP_BATCH = 32        # SB_WARP_BATCH: the images of one warp launch
 MASK_KINDS = ("none", "binary", "ramp", "random", "seam")
 GAIN_KINDS = ("none", "map1", "map3", "scalar", "vector")
 
 
-def seed_from_env():
-    s = os.environ.get("SB_RIG_FUZZ_SEED")
-    if not s:
-        return DEFAULT_SEED
-    seed = int(np.random.SeedSequence().entropy % (1 << 31)) if s == "random" else int(s)
-    print(f"rig fuzz: SB_RIG_FUZZ_SEED={seed}")
-    return seed
+seed_from_env = functools.partial(fuzz_chain.seed_from_env, "SB_RIG_FUZZ_SEED", DEFAULT_SEED)
 
 
 @dataclasses.dataclass
@@ -73,10 +68,11 @@ class Case:
     def scale(self):
         return np.float32(median([c.focal for c in self.cams]))  # Warper.set_scale, as float32 like the C ABI
 
+    def geometry(self):
+        return fuzz_chain.blend_geometry([r[:2] for r in self.rects], [r[2:] for r in self.rects], self.blender, self.strength)
+
     def roi(self):
-        x0 = min(r[0] for r in self.rects)
-        y0 = min(r[1] for r in self.rects)
-        return (x0, y0, max(r[0] + r[2] for r in self.rects) - x0, max(r[1] + r[3] for r in self.rects) - y0)
+        return self.geometry().roi
 
 
 # -- inputs -----------------------------------------------------------------------------------------------------------
@@ -216,9 +212,7 @@ def _rects(wtype, cams, sizes):
 
 def _strength(rng, rects, blender):
     """Blend strength aimed at a band count: 0, 1, 2, intermediate, the clipped maximum; or a blend width under 1."""
-    x0, y0 = min(r[0] for r in rects), min(r[1] for r in rects)
-    w = max(r[0] + r[2] for r in rects) - x0
-    h = max(r[1] + r[3] for r in rects) - y0
+    _, _, w, h = fuzz_chain.blend_geometry([r[:2] for r in rects], [r[2:] for r in rects]).roi
     root = math.sqrt(w * h)
     u = rng.random()
     if u < 0.06:
@@ -228,7 +222,7 @@ def _strength(rng, rects, blender):
     if u < 0.26:
         return 100.0                                                # far past the clip at ceil(log2(max side))
     nb = int(rng.choice([0, 0, 1, 1, 2, 2, 3, 4, 5]))
-    bw = 2.0 ** (nb + 1 + rng.uniform(0.1, 0.9))                    # blender.py:32: int(log2(bw) - 1) == nb
+    bw = 2.0 ** (nb + 1 + rng.uniform(0.1, 0.9))                    # Blender.prepare: int(log2(bw) - 1) == nb
     return _quant(max(1 / 256, bw * 100 / root))
 
 
@@ -289,7 +283,7 @@ def named(name, budget):
     side = budget["side"]
     if name == "flat_top":
         # a flat image whose rect is the top of the pano (no top padding) but whose padded rect reaches further below
-        # it than it is high: pyrDown level 0 is not NEAR (sb_pyrdown_fast.cu:228, second clause)
+        # it than it is high: pyrDown level 0 is not NEAR (launch_pyrdown_fast, the second clause of level 0's test)
         sizes = [(min(side, 90), 3), (min(side, 70), min(side, 40)), (min(side, 60), min(side, 30))]
         cams = [rigs.Camera(1, 1, 0, 0, np.array([[1, 0, 0.3], [0, 1, 36.0], [0, 0, 1]], np.float32)),
                 rigs.Camera(1, 1, 0, 0, np.array([[1, 0.1, 40.6], [0, 1, 9.25], [0, 0, 1]], np.float32)),
@@ -339,7 +333,7 @@ def named(name, budget):
         cams = [rigs.Camera(1, 1, 0, 0, np.array([[1, 0, ox], [0, 1, oy], [0, 0, 1]], np.float32)) for ox, oy in offs]
         c = Case(name, "affine", cams, sizes, "multiband", 0.0, ["none", "ramp"], ["none"] * 2, ["noise", "synth"], 17)
     elif name == "wide_feather":
-        # a feather image wider than 8192 px: the two-sweep distance-transform row kernel (sb_feather_fast.cu:271-272)
+        # a feather image wider than 8192 px: the two-sweep distance-transform row kernel (launch_feather_weights_fast)
         sizes = [(8300, 9), (700, 60)]
         cams = [rigs.Camera(1, 1, 0, 0, np.array([[1, 0, 0.5], [0, 1, 0.0], [0, 0, 1]], np.float32)),
                 rigs.Camera(1, 1, 0, 0, np.array([[1, 0, 4000.25], [0.02, 1, 4.5], [0, 0, 1]], np.float32))]
@@ -392,6 +386,19 @@ def gpu_set(seed):
     return _sets[("gpu", seed)]
 
 
+def ab_arrays(seed, ks):
+    """Cases `ks` of the GPU set through the compositor: the pano, its mask, every warped image and mask by name."""
+    cs = gpu_set(seed)
+    out = {}
+    for k in ks:
+        c = cs[k]
+        got = fuzz_chain.compositor_run(c, images(c), extras(c))
+        out[f"{k}_pano"], out[f"{k}_pmask"] = got["pano"], got["pmask"]
+        for i in range(c.n):
+            out[f"{k}_w{i}"], out[f"{k}_m{i}"] = got["warped"][i], got["masks"][i]
+    return out
+
+
 def emu_coverage(case):
     lanes, blocks = "SB_EMU_LANES" in case.env, "SB_EMU_BLOCKS" in case.env
     return coverage(case, pyr_fast=lanes, tile=blocks, dt_fast=lanes)
@@ -403,52 +410,25 @@ def redraw_share(cs):
 
 
 # -- the oracle side ----------------------------------------------------------------------------------------------------
-def oracle_run(O, case, imgs, ex, s16=False):
-    """The reference order of operations per image (stitcher.py:178-189, 219-225, 241-259): warp, compensator apply on
-    the warped image, blend mask = the caller's mask, or SeamFinder.resize(seam, warped mask), or the warped mask; then
-    Blender prepare / feed / blend.  `raw` holds the warped images and masks before compensation; s16: also the blend's
-    int16 result ("pano16")."""
+def oracle_run(O, case, imgs, ex, s16=False, crop=None):
+    """fuzz_chain.oracle_image per image, sliced by `crop`'s rects when given, then oracle_blend at the warped corners
+    and sizes or at the crop's corners and prepared sizes.  `rects` are the fed ones (corner, fed size), `raw` holds the
+    warped images and masks before slice and compensation; s16: also the blend's int16 result ("pano16")."""
     scale = case.scale()
-    warped, masks, corners, sizes, raw = [], [], [], [], []
-    for img, cam, (mask, seam, gain) in zip(imgs, case.cams, ex):
-        rect, wi, wm = O.warp(case.wtype, scale, Warper.get_K(cam, 1), cam.R, img)
-        raw.append((wi, wm))
-        if gain is not None:
-            wi = O.gain_apply(wi, gain)
-        if mask is not None:
-            wm = mask
-        elif seam is not None:
-            wm = O.seam_resize(seam, wm)
+    slices = crop.rects if crop is not None else [None] * case.n
+    raw, warped, masks, rects = [], [], [], []
+    for img, cam, sl, (mask, seam, gain) in zip(imgs, case.cams, slices, ex):
+        (rect, ri, rm), wi, wm = fuzz_chain.oracle_image(O, case.wtype, scale, Warper.get_K(cam, 1), cam.R, img, sl, gain,
+                                                         mask, seam)
+        raw.append((ri, rm))
         warped.append(wi)
         masks.append(wm)
-        corners.append(rect[:2])
-        sizes.append(rect[2:])
-    b = O.Blender(case.blender, case.strength)
-    b.prepare(corners, sizes)
-    for wi, wm, c in zip(warped, masks, corners):
-        b.feed(wi, wm, c)
-    pano16, pmask = b.blend_s16()
-    return dict(warped=warped, masks=masks, rects=[tuple(c) + tuple(s) for c, s in zip(corners, sizes)], roi=b.roi,
-                num_bands=b.num_bands if b._kind == "multiband" else -1, pano=O.convert_scale_abs(pano16), pmask=pmask,
-                raw=raw, pano16=pano16 if s16 else None)
-
-
-def compositor_run(Compositor, case, imgs, ex):
-    c = Compositor(case.cams, case.sizes, case.wtype, case.blender, case.strength)
-    try:
-        for i, (mask, seam, gain) in enumerate(ex):
-            if mask is not None:
-                c.set_mask(i, mask)
-            if seam is not None:
-                c.set_seam_mask(i, seam)
-            if gain is not None:
-                c.set_gain(i, gain)
-        pano, pmask = c.composite(imgs)
-        warped = [c.download_warped(i) for i in range(case.n)]
-        return dict(rects=list(c.rects), roi=tuple(c.roi), num_bands=c.num_bands, pano=pano, pmask=pmask,
-                    warped=[w for w, _ in warped], masks=[m for _, m in warped])
-    finally:
-        c.close()
+        rects.append(rect)
+    corners, sizes = (crop.corners, crop.sizes) if crop is not None else ([r[:2] for r in rects], [r[2:] for r in rects])
+    b, pano16, pmask = fuzz_chain.oracle_blend(O, case.blender, case.strength, corners, sizes, warped, masks)
+    return dict(warped=warped, masks=masks, rects=[tuple(c) + (wi.shape[1], wi.shape[0]) for c, wi in zip(corners, warped)],
+                roi=b.roi, num_bands=b.num_bands if b._kind == "multiband" else -1, pano=O.convert_scale_abs(pano16),
+                pmask=pmask, raw=raw, pano16=pano16 if s16 else None)
 
 
 def check(case, got, ref, seed):
@@ -468,26 +448,9 @@ def check(case, got, ref, seed):
 
 # -- coverage accounting ------------------------------------------------------------------------------------------------
 def plan(case):
-    """Blend kind, band count and the padded rects of a case, restated from sb_plan.cpp."""
-    x, y, w, h = case.roi()
-    bw = math.sqrt(w * h) * case.strength / 100.0  # derive_blend_params (sb_plan.cpp:32-47)
-    if case.blender == "no" or bw < 1.0:
-        return "no", 0, []
-    if case.blender == "feather":
-        return "feather", 0, []
-    nb = int(math.log(bw) / math.log(2.0) - 1.0)
-    nb = min(nb, int(math.ceil(math.log(max(w, h)) / math.log(2.0))))  # BlendPlan::set_geometry (sb_plan.cpp:67-76)
-    a, gap = 1 << nb, 3 << nb
-    wp, hp = -(-w // a) * a, -(-h // a) * a
-    padded = []
-    for (tx, ty, fw, fh) in case.rects:  # BlendPlan::add_feed (sb_plan.cpp:111-141)
-        x0, y0 = max(x, tx - gap), max(y, ty - gap)
-        x1, y1 = min(x + wp, tx + fw + gap), min(y + hp, ty + fh + gap)
-        x0 = x + (((x0 - x) >> nb) << nb)
-        y0 = y + (((y0 - y) >> nb) << nb)
-        ww, hh = -(-(x1 - x0) // a) * a, -(-(y1 - y0) // a) * a
-        padded.append(dict(w=fw, h=fh, top=ty - y0, pw=ww, ph=hh))
-    return "multiband", nb, padded
+    """Blend kind, band count and the padded feed rects of a case's rects (fuzz_chain.blend_geometry)."""
+    g = fuzz_chain.blend_geometry([r[:2] for r in case.rects], [r[2:] for r in case.rects], case.blender, case.strength)
+    return g.kind, g.nb, g.feeds
 
 
 def _z_nonpositive(case):
@@ -529,7 +492,7 @@ def coverage(case, pyr_fast=True, tile=True, dt_fast=True, pd_bin=True):
         tags.add("n>32")
     if _z_nonpositive(case):
         tags.add("z<=0")
-    # launch_warp (sb_warp.cu:457-463): maps or a 1-px source take k_warp_wide; else k_warp_rgbm<HAS_BM, ...>
+    # launch_warp: maps or a 1-px source take k_warp_wide; else k_warp_rgbm<HAS_BM, ...>
     has_bm = any(m != "none" or g != "none" for m, g in zip(case.masks, case.gains))
     tags.add("k_warp_wide" if case.wtype in MAP_TYPES else f"k_warp_rgbm<HAS_BM={int(has_bm)}>")
     if case.wtype in MAP_TYPES:
@@ -541,9 +504,9 @@ def coverage(case, pyr_fast=True, tile=True, dt_fast=True, pd_bin=True):
         tags.add("gray blend mask")
     if any(s[0] == 2 for s in case.sizes):
         tags.add("2-px source")
-    binary = pd_bin and all(m == "none" for m in case.masks)  # sb_compositor.cpp:215, 661, 693
+    binary = pd_bin and all(m == "none" for m in case.masks)  # use_blend_mask: set_mask / set_seam_mask turn it off
     if kind == "multiband" and pyr_fast:
-        for l in range(nb):  # launch_pyrdown_fast (sb_pyrdown_fast.cu:224-243)
+        for l in range(nb):  # launch_pyrdown_fast
             near = all((p["ph"] >> l) >= 4 for p in padded)
             if l == 0:
                 near = near and all(p["top"] <= p["h"] and p["ph"] - p["top"] - p["h"] <= p["h"] for p in padded)

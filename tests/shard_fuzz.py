@@ -16,12 +16,13 @@ coverage(case) turns them into tags a test can count.
 SB_SHARD_FUZZ_SEED=<int> or =random replaces the fixed default seed (the seed used is printed).
 """
 import dataclasses
+import functools
 import math
-import os
 from statistics import median
 
 import numpy as np
 
+import fuzz_chain
 import rig_fuzz
 from stitching_b200 import rigs
 from stitching_b200.warper import Warper
@@ -32,13 +33,7 @@ GPU = dict(side=400, area=160_000)        # H100: the oracle (scalar C on the CP
 WORLDS = (2, 3, 4, 5, 8)
 
 
-def seed_from_env():
-    s = os.environ.get("SB_SHARD_FUZZ_SEED")
-    if not s:
-        return DEFAULT_SEED
-    seed = int(np.random.SeedSequence().entropy % (1 << 31)) if s == "random" else int(s)
-    print(f"shard fuzz: SB_SHARD_FUZZ_SEED={seed}")
-    return seed
+seed_from_env = functools.partial(fuzz_chain.seed_from_env, "SB_SHARD_FUZZ_SEED", DEFAULT_SEED)
 
 
 @dataclasses.dataclass
@@ -139,8 +134,7 @@ def _extras(rng, n):
 def _mb_strength(rng, rects):
     """A multiband strength aimed at nb = 1, 2, an intermediate count or the clipped maximum (never 0: the sharded
     composite needs a band)."""
-    x0, y0 = min(r[0] for r in rects), min(r[1] for r in rects)
-    w, h = max(r[0] + r[2] for r in rects) - x0, max(r[1] + r[3] for r in rects) - y0
+    _, _, w, h = fuzz_chain.blend_geometry([r[:2] for r in rects], [r[2:] for r in rects]).roi
     if rng.random() < 0.15:
         return 400.0                                                # past the clip at ceil(log2(max side))
     nb = int(rng.choice([1, 1, 2, 2, 3, 4, 5]))
@@ -277,35 +271,20 @@ def named(name, budget=None):
     return c
 
 
-# -- the geometry, restated from sb_plan.cpp / sb_shard.cpp --------------------------------------------------------------
-def _feed_images(case, nb):
-    """FeedImage fields of BlendPlan::add_feed (multiband): padded origin px, py and size pw, ph, image offset inside."""
-    x, y, w, h = case.roi()
-    a, gap = 1 << nb, 3 << nb
-    wp, hp = -(-w // a) * a, -(-h // a) * a
-    out = []
-    for tx, ty, fw, fh in case.rects:
-        x0, y0 = max(x, tx - gap), max(y, ty - gap)
-        x1, y1 = min(x + wp, tx + fw + gap), min(y + hp, ty + fh + gap)
-        x0 = x + (((x0 - x) >> nb) << nb)
-        y0 = y + (((y0 - y) >> nb) << nb)
-        out.append(dict(px=x0 - x, py=y0 - y, pw=-(-(x1 - x0) // a) * a, ph=-(-(y1 - y0) // a) * a, left=tx - x0,
-                        top=ty - y0, w=fw, h=fh, dx=tx - x, dy=ty - y))
-    return out, wp, hp
-
-
+# -- the geometry, restated from the library's ShardPlan --------------------------------------------------------------
 def geometry(case):
     """Strip geometry of every rank, restated from the rig: dict(ok, kind, nb, axis, reversed, bounds, strips, empty,
     slab_levels (levels at which some slab is non-empty), has_slabs[r][l] (rank r receives a slab at level l))."""
-    kind, nb, _ = rig_fuzz.plan(case)
+    bg = case.geometry()
+    kind, nb = bg.kind, bg.nb
     n, world = case.n, case.world
-    x, y, w, h = case.roi()
+    x, y, w, h = bg.roi
     g = dict(kind=kind, nb=nb, axis=0, reversed=False, ok=n >= world and (kind == "feather" or (kind == "multiband" and nb >= 1)))
     if not g["ok"]:
         return g
     blocks = [block_of(n, world, r) for r in range(world)]
     if kind == "multiband":
-        imgs, wp, hp = _feed_images(case, nb)
+        imgs, (wp, hp) = bg.feeds, bg.padded
         a = 1 << nb
         snapped = []
         for r in range(1, world):
@@ -445,32 +424,23 @@ def coverage(case, tile=True):
 
 
 # -- the oracle side ----------------------------------------------------------------------------------------------------
-def _warp_all(O, case, imgs, ex):
-    scale = case.scale()
-    out = []
-    for img, cam, (mask, seam, gain) in zip(imgs, case.cams, ex):
-        rect, wi, wm = O.warp(case.wtype, scale, Warper.get_K(cam, 1), cam.R, img)
-        if gain is not None:
-            wi = O.gain_apply(wi, gain)
-        if mask is not None:
-            wm = mask
-        elif seam is not None:
-            wm = O.seam_resize(seam, wm)
-        out.append((rect, wi, wm))
-    return out
-
-
 def grouped_oracle(O, case, imgs, ex, world=None):
     """What every rank computes: per rank r, a blender that folds in the blocks of the lower ranks (each fed on its
     own, from 0), is fed r's images one at a time, folds in the blocks of the higher ranks, and blends.  Returns the
     warped images and masks, rects, roi, num_bands, and per rank the WHOLE blended panorama and mask (the rank keeps
     its strip of it, the test slices)."""
     world = case.world if world is None else world
-    warped = _warp_all(O, case, imgs, ex)
-    b0, panos = grouped_blend(O, case.blender, case.strength, [r[:2] for r, _, _ in warped], [wi for _, wi, _ in warped],
-                              [wm for _, _, wm in warped], world)
-    return dict(warped=[wi for _, wi, _ in warped], masks=[wm for _, _, wm in warped], rects=[tuple(r) for r, _, _ in warped],
-                roi=b0.roi, num_bands=b0.num_bands if b0._kind == "multiband" else -1, panos=panos)
+    scale = case.scale()
+    rects, warped, masks = [], [], []
+    for img, cam, (mask, seam, gain) in zip(imgs, case.cams, ex):
+        (rect, _, _), wi, wm = fuzz_chain.oracle_image(O, case.wtype, scale, Warper.get_K(cam, 1), cam.R, img, None, gain,
+                                                       mask, seam)
+        rects.append(tuple(rect))
+        warped.append(wi)
+        masks.append(wm)
+    b0, panos = grouped_blend(O, case.blender, case.strength, [r[:2] for r in rects], warped, masks, world)
+    return dict(warped=warped, masks=masks, rects=rects, roi=b0.roi, num_bands=b0.num_bands if b0._kind == "multiband" else -1,
+                panos=panos)
 
 
 def grouped_blend(O, kind, strength, corners, imgs, masks, world):
@@ -533,22 +503,19 @@ def cut(a, strip, axis):
 
 
 # -- the product side ---------------------------------------------------------------------------------------------------
-def hooks_run(Compositor, case, imgs, ex, copy):
-    """All ranks in this process: each sets the extras of its own images, uploads its block and runs phase 0; the
-    slabs are moved with `copy(dst, src, bytes)`; phase 1; strips and own warped images are downloaded."""
+def hooks_run(case, imgs, ex, copy, **compositor_kwargs):
+    """All ranks in this process (Compositor keywords `compositor_kwargs`: crop, input_sizes): each sets the extras of
+    its own images, uploads its block and runs phase 0; the slabs are moved with `copy(dst, src, bytes)`; phase 1;
+    strips and own warped images are downloaded."""
+    from stitching_b200 import Compositor
+
     ranks = []
     try:
         for r in range(case.world):
-            ranks.append(Compositor(case.cams, case.sizes, case.wtype, case.blender, case.strength, rank=r, world=case.world))
+            ranks.append(Compositor(case.cams, case.sizes, case.wtype, case.blender, case.strength, rank=r, world=case.world,
+                                    **compositor_kwargs))
         for c in ranks:
-            for i in range(c.first, c.first + c.count):
-                mask, seam, gain = ex[i]
-                if mask is not None:
-                    c.set_mask(i, mask)
-                if seam is not None:
-                    c.set_seam_mask(i, seam)
-                if gain is not None:
-                    c.set_gain(i, gain)
+            fuzz_chain.set_extras(c, ex, range(c.first, c.first + c.count))
             c.upload(imgs[c.first: c.first + c.count])
             c.shard_phase(0)
         sizes = {}
@@ -597,6 +564,22 @@ def check(case, got, slab_sizes, ref, seed):
         pano, pmask = ref["panos"][r]
         replay.assert_exact(rk["pano"], cut(pano, rk["strip"], rk["axis"]), f"{at}: strip {rk['strip']}")
         replay.assert_exact(rk["pmask"], cut(pmask, rk["strip"], rk["axis"]), f"{at}: strip mask")
+
+
+def ab_arrays(seed, ks):
+    """Cases `ks` of the GPU set, all ranks on this device: every rank's strip and its mask by name."""
+    from stitching_b200 import _lib
+
+    def copy(d, s, n):
+        _lib.check(_lib.lib().sb_device_copy(d, s, n), "sb_device_copy")
+
+    cs = gpu_set(seed)
+    out = {}
+    for k in ks:
+        got, _ = hooks_run(cs[k], rig_fuzz.images(cs[k]), rig_fuzz.extras(cs[k]), copy)
+        for r, g in enumerate(got):
+            out[f"{k}_{r}_pano"], out[f"{k}_{r}_pmask"] = g["pano"], g["pmask"]
+    return out
 
 
 def assemble(got):

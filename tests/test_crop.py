@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import crop_fuzz
+import fuzz_chain
 import rig_fuzz
 from conftest import ROOT
 from stitching_b200 import Crop, StitchingError
@@ -47,7 +48,7 @@ def test_full_crop_equals_no_crop(use_emu, oracle):
     cc = crop_fuzz.named("full", rig_fuzz.EMU)
     imgs, ex = rig_fuzz.images(cc.case), rig_fuzz.extras(cc.case)
     got = crop_fuzz.run_and_check(oracle, cc, SEED)
-    plain = rig_fuzz.compositor_run(crop_fuzz.Compositor, cc.case, imgs, ex)
+    plain = fuzz_chain.compositor_run(cc.case, imgs, ex)
     assert got["num_bands"] == plain["num_bands"]
     assert np.array_equal(got["pano"], plain["pano"]) and np.array_equal(got["pmask"], plain["pmask"])
 

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import dropin_fuzz
+import fuzz_chain
 import rig_fuzz
 from stitching_b200 import Compositor, StitchingError, _lib, rigs
 
@@ -37,7 +38,7 @@ def test_dropin_fuzz_coverage(oracle):
 def _compositor_vs_oracle(oracle, case):
     imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(case)
     ref = rig_fuzz.oracle_run(oracle, case, imgs, ex)
-    got = rig_fuzz.compositor_run(Compositor, case, imgs, ex)
+    got = fuzz_chain.compositor_run(case, imgs, ex)
     rig_fuzz.check(case, got, ref, "strength")
 
 

@@ -8,6 +8,7 @@ import pytest
 
 import crop_fuzz
 import final_scale
+import fuzz_chain
 import rig_fuzz
 import shard_fuzz
 from stitching_b200 import Compositor, StitchingError
@@ -109,7 +110,7 @@ def test_equal_input_sizes_change_nothing(use_emu, oracle):
     out, launches = [], []
     for kw in ({}, {"input_sizes": case.sizes}):
         before = use_emu.sb_launch_count()
-        out.append(final_scale.compositor_run(case, imgs, ex, **kw))
+        out.append(fuzz_chain.compositor_run(case, imgs, ex, **kw))
         launches.append(use_emu.sb_launch_count() - before)
     rig_fuzz.check(case, out[1], out[0], SEED)
     assert launches[0] == launches[1], launches

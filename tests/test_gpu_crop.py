@@ -2,14 +2,12 @@
 the full crop against no crop, submit / wait against composite(), the A/B switches, and the sharded roles on one GPU."""
 import ctypes as C
 import os
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 
 import crop_fuzz
+import fuzz_chain
 import rig_fuzz
 
 pytestmark = pytest.mark.gpu
@@ -46,8 +44,8 @@ def test_crop_fuzz_coverage_on_the_gpu():
 def test_full_crop_equals_no_crop(cuda_lib):
     cc = crop_fuzz.named("full", rig_fuzz.GPU)
     imgs, ex = rig_fuzz.images(cc.case), rig_fuzz.extras(cc.case)
-    got = crop_fuzz.compositor_run(cc, imgs, ex)
-    plain = rig_fuzz.compositor_run(crop_fuzz.Compositor, cc.case, imgs, ex)
+    got = fuzz_chain.compositor_run(cc.case, imgs, ex, crop=cc.crop)
+    plain = fuzz_chain.compositor_run(cc.case, imgs, ex)
     assert np.array_equal(got["pano"], plain["pano"]) and np.array_equal(got["pmask"], plain["pmask"])
 
 
@@ -79,47 +77,14 @@ def test_submit_wait_with_a_crop_equals_composite(cuda_lib):
         c.close()
 
 
-_CHILD = """
-import sys
-import numpy as np
-sys.path.insert(0, sys.argv[1]); sys.path.insert(0, sys.argv[1] + "/tests")
-import crop_fuzz, rig_fuzz
-from stitching_b200 import _lib
-_lib.check(_lib.lib().sb_init(0), "sb_init")
-cs = crop_fuzz.cases(int(sys.argv[3]), int(sys.argv[5]), rig_fuzz.GPU)
-out = {}
-for k in map(int, sys.argv[4].split(",")):
-    c = cs[k]
-    got = crop_fuzz.compositor_run(c, rig_fuzz.images(c.case), rig_fuzz.extras(c.cropped_case()))
-    out[f"{k}_pano"], out[f"{k}_pmask"] = got["pano"], got["pmask"]
-np.savez(sys.argv[2], **out)
-"""
-
-
 def test_ab_switches_with_a_crop_give_identical_bytes(cuda_lib):
-    from conftest import ROOT
-
     cs = gpu_set()[:GPU_COUNT]
     picked = sorted({cs.index(_multiband_crop(cs)),
                      next(k for k, c in enumerate(cs) if rig_fuzz.plan(c.cropped_case())[1] >= 3),
                      next(k for k, c in enumerate(cs) if any(m in ("ramp", "random", "seam") for m in c.case.masks)),
                      next(k for k, c in enumerate(cs) if rig_fuzz.plan(c.cropped_case())[0] == "feather")})
-    res = {}
-    with tempfile.TemporaryDirectory() as d:
-        for key in (None, "SB_TILE", "SB_PD_BIN", "SB_SRC4", "SB_GRAPH"):
-            env = {k: v for k, v in os.environ.items() if not (k.startswith("SB_") and k != "SB_CROP_FUZZ_SEED")}
-            if key:
-                env[key] = "0"
-            out = os.path.join(d, f"{key or 'defaults'}.npz")
-            subprocess.check_call([sys.executable, "-c", _CHILD, ROOT, out, str(SEED), ",".join(map(str, picked)), str(GPU_COUNT)],
-                                  env=env)
-            with np.load(out) as z:
-                res[key] = {k: z[k] for k in z.files}
-    base = res.pop(None)
-    for key, arrays in res.items():
-        assert arrays.keys() == base.keys()
-        for name, a in arrays.items():
-            assert np.array_equal(a, base[name]), f"{key}=0: {name} differs"
+    fuzz_chain.ab_run("crop_fuzz:ab_arrays", [SEED, GPU_COUNT, picked],
+                      [("SB_TILE", "0"), ("SB_PD_BIN", "0"), ("SB_SRC4", "0"), ("SB_GRAPH", "0")], "SB_CROP_FUZZ_SEED")
 
 
 def _device_copy(d, s, n):

@@ -3,10 +3,9 @@ against the CPU oracle, and every panorama equal to the fused Compositor's for t
 import numpy as np
 import pytest
 
-import crop_fuzz
 import dropin_fuzz
+import fuzz_chain
 import rig_fuzz
-from stitching_b200 import Compositor
 
 pytestmark = pytest.mark.gpu
 
@@ -17,7 +16,7 @@ SEED = dropin_fuzz.seed_from_env()
 def test_dropin_fuzz_against_oracle_and_compositor(cuda_lib, oracle, k):
     dc = dropin_fuzz.gpu_set(SEED)[k]
     imgs, ex, got = dropin_fuzz.run_and_check(oracle, dc, SEED)
-    fused = crop_fuzz.compositor_run(dc.crop, imgs, ex) if dc.crop is not None else rig_fuzz.compositor_run(Compositor, dc.case, imgs, ex)
+    fused = fuzz_chain.compositor_run(dc.case, imgs, ex, crop=dc.crop.crop if dc.crop is not None else None)
     assert np.array_equal(fused["pano"], got["pano"]) and np.array_equal(fused["pmask"], got["pmask"]), \
         f"{dc.describe()}: the drop-in panorama differs from the compositor's"
 

@@ -2,20 +2,16 @@
 shard draws against the compositor fed resized frames, the reference Stitcher's final_megapix records replayed from
 the camera views, SB_SRC4=0 in a child process, and one 48 MP camera."""
 import ctypes as C
-import os
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 
 import crop_fuzz
 import final_scale
+import fuzz_chain
 import reference_cases as RC
 import rig_fuzz
 import shard_fuzz
-from conftest import ROOT
 from stitching_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -89,32 +85,8 @@ def test_dropin_resize_reproduces_the_record(cuda_lib, name):
     final_scale.resized_check(images.resize_exact, z, _record_views(name))
 
 
-_CHILD = """
-import sys
-sys.path[:0] = [sys.argv[1], sys.argv[1] + "/tests"]
-import numpy as np
-import final_scale, reference_cases as RC
-from stitching_b200 import _lib
-_lib.check(_lib.lib().sb_init(0), "sb_init")
-z = final_scale.record(sys.argv[3])
-c = final_scale.compositor(z)
-pano, mask = c.composite(final_scale.views(z))
-np.savez(sys.argv[2], pano=pano, mask=mask, warped=np.concatenate([np.concatenate([a.ravel(), b.ravel()]) for a, b in (c.download_warped(i) for i in range(c.n))]))
-"""
-
-
 def test_packed_sources_are_identical(cuda_lib):
     """SB_SRC4=0 (the resize writes packed FINAL sources, the warp reads them) in a child process: the same panorama,
     mask and warped images as the word layout, on record 5."""
-    res = {}
-    with tempfile.TemporaryDirectory() as d:
-        for flag in ("1", "0"):
-            out = os.path.join(d, f"{flag}.npz")
-            env = {k: v for k, v in os.environ.items() if not k.startswith("SB_")}
-            env["SB_SRC4"] = flag
-            subprocess.check_call([sys.executable, "-c", _CHILD, ROOT, out, "5"], env=env, timeout=900)
-            with np.load(out) as z:
-                res[flag] = {k: z[k] for k in z.files}
-    for k in res["1"]:
-        assert np.array_equal(res["1"][k], res["0"][k]), k
-    assert RC.digest(res["0"]["pano"]) == str(final_scale.record("5")["pano"])
+    base = fuzz_chain.ab_run("final_scale:ab_arrays", ["5"], [("SB_SRC4", "0")], "SB_FINAL_SCALE_SEED", timeout=900)
+    assert RC.digest(base["pano"]) == str(final_scale.record("5")["pano"])

@@ -294,33 +294,25 @@ def test_setters_between_pipelined_submits(cuda_lib):
     test_host_logic.check_setters_between_submits(4)
 
 
+def simple_kernels_panorama():
+    """cfg 2 at a quarter of its size through the compositor: the panorama and its mask."""
+    cfg = rigs.config("cfg2", 4)
+    cams = cfg["cameras"]
+    imgs = [rigs.noise_image(cfg["h"], cfg["w"], 300 + i) for i in range(len(cams))]
+    c = Compositor(cams, [(cfg["w"], cfg["h"])] * len(cams), cfg["warper"], cfg["blender"], cfg["strength"])
+    try:
+        p, m = c.composite(imgs)
+        return dict(p=p, m=m)
+    finally:
+        c.close()
+
+
 def test_simple_and_fast_kernels_agree(cuda_lib):
-    """A/B inside one process is not possible (the variant is chosen once per process): run the other variant in
-    a child process and compare panoramas byte for byte."""
-    import subprocess
-    import sys
-    import tempfile
+    """A/B inside one process is not possible (the variant is chosen once per process): the fast kernels (the default)
+    and SB_KERNELS=simple each run in a child process and their panoramas must agree byte for byte."""
+    import fuzz_chain
 
-    code = (
-        "import sys, numpy as np; sys.path.insert(0, sys.argv[1]);"
-        "from stitching_b200 import Compositor, rigs;"
-        "cfg = rigs.config('cfg2', 4); cams = cfg['cameras'];"
-        "imgs = [rigs.noise_image(cfg['h'], cfg['w'], 300 + i) for i in range(len(cams))];"
-        "c = Compositor(cams, [(cfg['w'], cfg['h'])] * len(cams), cfg['warper'], cfg['blender'], cfg['strength']);"
-        "p, m = c.composite(imgs); np.savez(sys.argv[2], p=p, m=m)"
-    )
-    from conftest import ROOT
-
-    res = {}
-    with tempfile.TemporaryDirectory() as d:
-        for variant in ("simple", "fast"):
-            env = dict(os.environ)
-            env["SB_KERNELS"] = variant
-            out = os.path.join(d, variant + ".npz")
-            subprocess.check_call([sys.executable, "-c", code, ROOT, out], env=env)
-            z = np.load(out)
-            res[variant] = (z["p"], z["m"])
-    assert np.array_equal(res["simple"][0], res["fast"][0]) and np.array_equal(res["simple"][1], res["fast"][1])
+    fuzz_chain.ab_run("test_gpu_parity:simple_kernels_panorama", [], [("SB_KERNELS", "simple")])
 
 
 def test_full_size_properties(cuda_lib, oracle):

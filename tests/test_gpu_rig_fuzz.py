@@ -1,15 +1,9 @@
 """Seeded random rigs (tests/rig_fuzz.py) through the compositor on the GPU, bit for bit against the CPU oracle, and the
 A/B environment switches of the library, each of which must give the same bytes as the defaults."""
-import os
-import subprocess
-import sys
-import tempfile
-
-import numpy as np
 import pytest
 
+import fuzz_chain
 import rig_fuzz
-from stitching_b200 import Compositor
 
 pytestmark = pytest.mark.gpu
 
@@ -21,7 +15,7 @@ def test_rig_fuzz_against_oracle(cuda_lib, oracle, k):
     case = rig_fuzz.gpu_set(SEED)[k]
     imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(case)
     ref = rig_fuzz.oracle_run(oracle, case, imgs, ex)
-    got = rig_fuzz.compositor_run(Compositor, case, imgs, ex)
+    got = fuzz_chain.compositor_run(case, imgs, ex)
     rig_fuzz.check(case, got, ref, SEED)
 
 
@@ -45,24 +39,6 @@ def test_rig_fuzz_coverage_on_the_gpu(oracle):
 SWITCHES = [("SB_TILE", "0"), ("SB_TILE_MAXL", "3"), ("SB_GRAPH", "0"), ("SB_PDL", "0"), ("SB_DT", "0"), ("SB_PD_BIN", "0"),
             ("SB_SRC4", "0")]
 
-_CHILD = """
-import sys
-import numpy as np
-sys.path.insert(0, sys.argv[1]); sys.path.insert(0, sys.argv[1] + "/tests")
-import rig_fuzz
-from stitching_b200 import Compositor, _lib
-_lib.check(_lib.lib().sb_init(0), "sb_init")
-cs = rig_fuzz.gpu_set(int(sys.argv[3]))
-out = {}
-for k in map(int, sys.argv[4].split(",")):
-    c = cs[k]
-    got = rig_fuzz.compositor_run(Compositor, c, rig_fuzz.images(c), rig_fuzz.extras(c))
-    out[f"{k}_pano"], out[f"{k}_pmask"] = got["pano"], got["pmask"]
-    for i in range(c.n):
-        out[f"{k}_w{i}"], out[f"{k}_m{i}"] = got["warped"][i], got["masks"][i]
-np.savez(sys.argv[2], **out)
-"""
-
 
 def _ab_cases(cs):
     """About six cases for the switches: multiband with at least 4 bands (tile levels 2 and 3 under SB_TILE_MAXL=3) with
@@ -82,24 +58,7 @@ def _ab_cases(cs):
 
 
 def test_ab_switches_give_identical_bytes(cuda_lib):
-    from conftest import ROOT
-
     cs = rig_fuzz.gpu_set(SEED)
     picked = _ab_cases(cs)
-    print("A/B cases: " + "; ".join(cs[k].describe() for k in picked))
-    res = {}
-    with tempfile.TemporaryDirectory() as d:
-        for key, val in [(None, None)] + SWITCHES:
-            env = {k: v for k, v in os.environ.items() if not (k.startswith("SB_") and k != "SB_RIG_FUZZ_SEED")}
-            if key:
-                env[key] = val
-            out = os.path.join(d, f"{key or 'defaults'}.npz")
-            subprocess.check_call([sys.executable, "-c", _CHILD, ROOT, out, str(SEED), ",".join(map(str, picked))], env=env)
-            with np.load(out) as z:
-                res[key] = {k: z[k] for k in z.files}
-    base = res.pop(None)
-    for key, arrays in res.items():
-        assert arrays.keys() == base.keys()
-        for name, a in arrays.items():
-            k = int(name.split("_")[0])
-            assert np.array_equal(a, base[name]), f"{key}={dict(SWITCHES)[key]}: {name} differs ({cs[k].describe()})"
+    print("A/B cases: " + "; ".join(f"{k}: {cs[k].describe()}" for k in picked))
+    fuzz_chain.ab_run("rig_fuzz:ab_arrays", [SEED, picked], SWITCHES, "SB_RIG_FUZZ_SEED")

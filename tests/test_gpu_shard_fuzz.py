@@ -3,18 +3,14 @@ ranks' groups: all ranks on one device with the slabs moved by device copies thr
 strips under the A/B switches SB_TILE=0 and SB_PD_BIN=0; and, with two or more GPUs, the real exchange (IPC pushes and
 the NCCL fallback) through sb_compositor_run."""
 import os
-import subprocess
-import sys
-import tempfile
 
-import numpy as np
 import pytest
 
+import fuzz_chain
 import rig_fuzz
 import shard_fuzz
 import torchrun_job
 from conftest import ROOT
-from stitching_b200 import Compositor
 
 pytestmark = pytest.mark.gpu
 
@@ -32,7 +28,7 @@ def test_shard_fuzz_on_one_gpu(cuda_lib, oracle, k):
     case = shard_fuzz.gpu_set(SEED)[k]
     imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(case)
     ref = shard_fuzz.grouped_oracle(oracle, case, imgs, ex)
-    got, sizes = shard_fuzz.hooks_run(Compositor, case, imgs, ex, _device_copy)
+    got, sizes = shard_fuzz.hooks_run(case, imgs, ex, _device_copy)
     shard_fuzz.check(case, got, sizes, ref, SEED)
 
 
@@ -50,25 +46,6 @@ def test_shard_fuzz_coverage_on_the_gpu(oracle):
 
 
 # -- A/B switches: read once per process, so each setting runs in a child process --------------------------------------
-_CHILD = """
-import sys
-import numpy as np
-sys.path.insert(0, sys.argv[1]); sys.path.insert(0, sys.argv[1] + "/tests")
-import rig_fuzz, shard_fuzz
-from stitching_b200 import Compositor, _lib
-_lib.check(_lib.lib().sb_init(0), "sb_init")
-copy = lambda d, s, n: _lib.check(_lib.lib().sb_device_copy(d, s, n), "sb_device_copy")
-cs = shard_fuzz.gpu_set(int(sys.argv[3]))
-out = {}
-for k in map(int, sys.argv[4].split(",")):
-    c = cs[k]
-    got, _ = shard_fuzz.hooks_run(Compositor, c, rig_fuzz.images(c), rig_fuzz.extras(c), copy)
-    for r, g in enumerate(got):
-        out[f"{k}_{r}_pano"], out[f"{k}_{r}_pmask"] = g["pano"], g["pmask"]
-np.savez(sys.argv[2], **out)
-"""
-
-
 def _ab_cases(cs):
     """Multiband with slabs at the tile levels, with and without gray masks, and a feather rig."""
     tile = [k for k, c in enumerate(cs) if c.blender == "multiband" and "tile l0 with slab items" in shard_fuzz.coverage(c)]
@@ -81,23 +58,9 @@ def _ab_cases(cs):
 def test_shard_ab_switches_give_identical_strips(cuda_lib):
     cs = shard_fuzz.gpu_set(SEED)
     picked = _ab_cases(cs)
-    print("A/B cases: " + "; ".join(cs[k].describe() for k in picked))
-    res = {}
-    with tempfile.TemporaryDirectory() as d:
-        for key, val in [(None, None), ("SB_TILE", "0"), ("SB_PD_BIN", "0")]:
-            env = {k: v for k, v in os.environ.items() if not (k.startswith("SB_") and k != "SB_SHARD_FUZZ_SEED")}
-            if key:
-                env[key] = val
-            out = os.path.join(d, f"{key or 'defaults'}.npz")
-            subprocess.check_call([sys.executable, "-c", _CHILD, ROOT, out, str(SEED), ",".join(map(str, picked))], env=env,
-                                  timeout=900)
-            with np.load(out) as z:
-                res[key] = {k: z[k] for k in z.files}
-    base = res.pop(None)
-    for key, arrays in res.items():
-        assert arrays.keys() == base.keys()
-        for name, a in arrays.items():
-            assert np.array_equal(a, base[name]), f"{key}=0: {name} differs ({cs[int(name.split('_')[0])].describe()})"
+    print("A/B cases: " + "; ".join(f"{k}: {cs[k].describe()}" for k in picked))
+    fuzz_chain.ab_run("shard_fuzz:ab_arrays", [SEED, picked], [("SB_TILE", "0"), ("SB_PD_BIN", "0")], "SB_SHARD_FUZZ_SEED",
+                      timeout=900)
 
 
 # -- two or more GPUs: the real exchange ----------------------------------------------------------------------------------
@@ -106,7 +69,7 @@ import os, sys
 sys.path.insert(0, sys.argv[1]); sys.path.insert(0, os.path.join(sys.argv[1], "tests"))
 import numpy as np
 import torch.distributed as dist
-import rig_fuzz, shard_fuzz
+import fuzz_chain, rig_fuzz, shard_fuzz
 from stitching_b200 import Compositor
 from stitching_b200 import dist as sbdist
 
@@ -118,14 +81,7 @@ for k in ks:
     case = cs[k]
     imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(case)
     c = Compositor(case.cams, case.sizes, case.wtype, case.blender, case.strength, rank=rank, world=world)
-    for i in range(c.first, c.first + c.count):
-        mask, seam, gain = ex[i]
-        if mask is not None:
-            c.set_mask(i, mask)
-        if seam is not None:
-            c.set_seam_mask(i, seam)
-        if gain is not None:
-            c.set_gain(i, gain)
+    fuzz_chain.set_extras(c, ex, range(c.first, c.first + c.count))
     c.upload(imgs[c.first: c.first + c.count])
     for _ in range(3):           # repeated steps reuse the slab buffers and the step-counted flags
         c.run()

@@ -1,14 +1,10 @@
 """Timelapse frames from the fused compositor on the H100: the reference Stitcher's recorded timelapse run replayed from
 its camera views, random rigs / crops / resized inputs / gains against the oracle, the A/B switches in child processes,
 and the drop-in chain (Warper.warp_image -> slice -> apply_gain -> Timelapser) on the same rig."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
+import fuzz_chain
 import reference_cases as RC
 import replay
 import rig_fuzz
@@ -19,7 +15,6 @@ pytestmark = pytest.mark.gpu
 
 SEED = TF.seed_from_env()
 COUNT = 150
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 _sets = {}
 
@@ -104,13 +99,8 @@ AB_CASES = list(range(0, 24, 3)) + [COUNT, COUNT + 1]
 
 @pytest.mark.parametrize("env", [{"SB_GRAPH": "0"}, {"SB_SRC4": "0"}], ids=["SB_GRAPH=0", "SB_SRC4=0"])
 def test_ab_switches_give_identical_frames(cuda_lib, env):
-    code = ("import json, sys; sys.path[:0] = [%r, %r]; from stitching_b200 import _lib; _lib.check(_lib.lib().sb_init(0)); "
-            "import rig_fuzz, timelapse_fuzz as TF; print(json.dumps(TF.frame_digests(%d, %d, %r, rig_fuzz.GPU)))"
-            % (ROOT, os.path.join(ROOT, "tests"), SEED, COUNT, AB_CASES))
-    out = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **env), capture_output=True, text=True, timeout=1800)
-    assert out.returncode == 0, out.stderr[-3000:]
-    child = json.loads(out.stdout.strip().splitlines()[-1])
-    assert child == TF.frame_digests(SEED, COUNT, AB_CASES, rig_fuzz.GPU)
+    fuzz_chain.ab_run("timelapse_fuzz:frame_digests", [SEED, COUNT, AB_CASES, rig_fuzz.GPU], list(env.items()),
+                      "SB_TIMELAPSE_FUZZ_SEED")
 
 
 def test_equals_dropin_chain(cuda_lib):

@@ -9,6 +9,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import fuzz_chain
 import replay
 import rig_fuzz
 from stitching_b200 import Blender, Compositor, StitchingError, Warper, rigs
@@ -624,7 +625,7 @@ def test_rig_fuzz_against_oracle(use_emu, oracle, monkeypatch, k):
         monkeypatch.setenv(key, v)
     imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(case)
     ref = rig_fuzz.oracle_run(oracle, case, imgs, ex)
-    got = rig_fuzz.compositor_run(Compositor, case, imgs, ex)
+    got = fuzz_chain.compositor_run(case, imgs, ex)
     rig_fuzz.check(case, got, ref, _EMU_SEED)
 
 

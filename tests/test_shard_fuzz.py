@@ -30,7 +30,7 @@ def test_shard_fuzz_against_grouped_oracle(use_emu, oracle, monkeypatch, k):
         monkeypatch.setenv(key, v)
     imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(case)
     ref = shard_fuzz.grouped_oracle(oracle, case, imgs, ex)
-    got, sizes = shard_fuzz.hooks_run(Compositor, case, imgs, ex, _memmove)
+    got, sizes = shard_fuzz.hooks_run(case, imgs, ex, _memmove)
     shard_fuzz.check(case, got, sizes, ref, SEED)
 
 

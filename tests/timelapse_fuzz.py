@@ -8,15 +8,16 @@ rig_fuzz rigs (no crop) and crop_fuzz crops, camera frames resized on the device
 form of gain; the oracle is the warp, the numpy slice, oracle.gain_apply and oracle.Timelapser.  Rects, canvas and every
 frame are compared bit for bit.
 
-SB_TIMELAPSE_FUZZ_SEED=<int> replaces the fixed default seed.
+SB_TIMELAPSE_FUZZ_SEED=<int> or =random replaces the fixed default seed (the seed used is printed).
 """
 import dataclasses
-import os
+import functools
 
 import numpy as np
 
 import crop_fuzz
 import final_scale
+import fuzz_chain
 import replay
 import rig_fuzz
 from stitching_b200 import Compositor
@@ -25,9 +26,7 @@ DEFAULT_SEED = 20261020
 KINDS = ("as_is", "crop")
 
 
-def seed_from_env():
-    s = os.environ.get("SB_TIMELAPSE_FUZZ_SEED")
-    return int(s) if s else DEFAULT_SEED
+seed_from_env = functools.partial(fuzz_chain.seed_from_env, "SB_TIMELAPSE_FUZZ_SEED", DEFAULT_SEED)
 
 
 @dataclasses.dataclass
@@ -110,12 +109,8 @@ def oracle_run(O, tc, imgs, gs):
     t.initialize(*tc.prepared())
     frames = []
     for i, (img, cam, gain) in enumerate(zip(imgs, case.cams, gs)):
-        _, wi, _ = O.warp(case.wtype, scale, rig_fuzz.Warper.get_K(cam, 1), cam.R, img, want_mask=False)
-        if tc.crop is not None:
-            x, y, w, h = tc.crop.rects[i]
-            wi = np.ascontiguousarray(wi[y:y + h, x:x + w])
-        if gain is not None:
-            wi = O.gain_apply(wi, gain)
+        _, wi, _ = fuzz_chain.oracle_image(O, case.wtype, scale, rig_fuzz.Warper.get_K(cam, 1), cam.R, img,
+                                           tc.crop.rects[i] if tc.crop is not None else None, gain, want_mask=False)
         t.process_frame(wi, fed[i][:2])
         frames.append(t.get_frame())
     return dict(rects=fed, roi=tuple(t.roi), frames=frames)
@@ -164,18 +159,17 @@ def run_and_check(O, tc, seed):
 
 
 def frame_digests(seed, count, ks, budget):
-    """Digests of every frame of cases `ks` of cases(seed, count, budget) (the ones with a canvas) on the device of this
-    process: what a child process under an A/B switch prints for its parent to compare."""
+    """Case index -> the digests of every frame, for cases `ks` of cases(seed, count, budget) with a canvas."""
     import reference_cases as RC
 
-    out = []
+    out = {}
     cs = cases(seed, count, budget)
     for k in ks:
         tc = cs[k]
         if 0 in canvas(tc)[2:]:
             continue
         got = compositor_run(tc, frames_in(tc), gains(tc))
-        out.append([RC.digest(f) for f in got["frames"]])
+        out[k] = [RC.digest(f) for f in got["frames"]]
     return out
 
 
@@ -241,8 +235,7 @@ def canvas(tc):
 def canvas_of(kind, corners, sizes):
     """Timelapser.initialize's roi: resultRoi, or resultRoiIntersection built as cv::Rect(tl, br)."""
     if kind == "as_is":
-        x0, y0 = min(c[0] for c in corners), min(c[1] for c in corners)
-        return (x0, y0, max(c[0] + s[0] for c, s in zip(corners, sizes)) - x0, max(c[1] + s[1] for c, s in zip(corners, sizes)) - y0)
+        return fuzz_chain.blend_geometry(corners, sizes).roi
     tlx, tly = max(c[0] for c in corners), max(c[1] for c in corners)
     brx, bry = min(c[0] + s[0] for c, s in zip(corners, sizes)), min(c[1] + s[1] for c, s in zip(corners, sizes))
     return (min(tlx, brx), min(tly, bry), abs(brx - tlx), abs(bry - tly))
