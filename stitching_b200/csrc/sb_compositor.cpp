@@ -94,9 +94,6 @@ struct sb_compositor {
     // multi-GPU: this process composites images [first, first + count) and one column strip of the panorama
     bool sharded = false;
     int first = 0, count = 0;
-    // the slab exchange runs on its own stream, in two parts, beside the kernels (see compositor_enqueue_kernels)
-    cudaStream_t comm_stream = nullptr;
-    cudaEvent_t e_part[2] = {}, e_xchg[2] = {};  // partial sums of part k written / part k received
     ShardPlan shard;
     // timelapse mode: no blend plan; every step writes one frame of the canvas per image (cv.detail.Timelapser)
     int timelapse = 0;                 // 0, SB_TIMELAPSE_AS_IS or SB_TIMELAPSE_CROP
@@ -169,18 +166,13 @@ static void compositor_free(sb_compositor *c)
 {
     if (!c) return;
     cudaStream_t s = c->stream ? c->stream : default_stream();
-    for (cudaStream_t q : {c->stream, c->h2d, c->d2h, c->comm_stream})  // nothing queued may still use what is freed
+    for (cudaStream_t q : {c->stream, c->h2d, c->d2h})  // nothing queued may still use what is freed
         if (q) (void)cudaStreamSynchronize(q);
     for (Slot &sl : c->slots) slot_free(sl, s);
     for (Image &im : c->img) image_free(im, s);
     dev_free(c->flush_buf, s);
     if (c->h2d) (void)cudaStreamDestroy(c->h2d);
     if (c->d2h) (void)cudaStreamDestroy(c->d2h);
-    if (c->comm_stream) (void)cudaStreamDestroy(c->comm_stream);
-    for (int k = 0; k < 2; ++k) {
-        if (c->e_part[k]) (void)cudaEventDestroy(c->e_part[k]);
-        if (c->e_xchg[k]) (void)cudaEventDestroy(c->e_xchg[k]);
-    }
     for (auto &e : c->tev) (void)cudaEventDestroy(e);
     c->shard.release(s);
     c->plan.release(s);
@@ -554,41 +546,26 @@ static int compositor_enqueue(sb_compositor *c, bool events, int slot = 0)
     return compositor_enqueue_kernels(c, events, slot);
 }
 
-// sharded step: pyrDown of level l -> l+1 for the own images
-static int shard_pyrdown(sb_compositor *c, cudaStream_t s, int l)
+// sharded step, exchange part `part` (sb_shard.h): what its partial sums read, for the own images -- the feather weights,
+// or the pyrDowns to the part's levels
+template <class Mark>
+static int shard_local(sb_compositor *c, int part, cudaStream_t s, const Mark &mark)
 {
     BlendPlan &P = c->plan;
+    if (P.kind == SB_BLEND_FEATHER) {
+        SB_TRY(launch_feather_weights(P.imgs_dev + c->first, P.imgs.data() + c->first, c->count, P.sharpness, s));
+        return mark("feather_weights");
+    }
     const int n = (int)P.imgs.size();
-    int mw = 0, mh = 0;
-    for (int i = c->first; i < c->first + c->count; ++i) {
-        mw = std::max(mw, P.imgs[i].pw >> (l + 1));
-        mh = std::max(mh, P.imgs[i].ph >> (l + 1));
-    }
-    return launch_pyrdown(P.imgs_dev, P.imgs.data(), P.pyr_dev + (size_t)l * n, c->first, c->count, l, mw, mh, s, P.binary_masks);
-}
-
-// sharded step, local part: pyramids of the own images, then the partial sums every neighbour needs
-static int shard_feather_weights(sb_compositor *c, cudaStream_t s)
-{
-    BlendPlan &P = c->plan;
-    return launch_feather_weights(P.imgs_dev + c->first, P.imgs.data() + c->first, c->count, P.sharpness, s);
-}
-
-static int shard_local(sb_compositor *c, cudaStream_t s, const std::function<int(const std::string &)> &mark)
-{
-    if (c->plan.kind == SB_BLEND_FEATHER) {
-        SB_TRY(shard_feather_weights(c, s));
-        SB_TRY(mark("feather_weights"));
-        SB_TRY(c->shard.feather_partial_out(c->plan, s));
-        SB_TRY(mark("partial_out"));
-        return SB_OK;
-    }
-    for (int l = 0; l < c->plan.nb; ++l) {
-        SB_TRY(shard_pyrdown(c, s, l));
+    for (int l = part == 0 ? 0 : 1; l < (part == 0 ? 1 : P.nb); ++l) {
+        int mw = 0, mh = 0;
+        for (int i = c->first; i < c->first + c->count; ++i) {
+            mw = std::max(mw, P.imgs[i].pw >> (l + 1));
+            mh = std::max(mh, P.imgs[i].ph >> (l + 1));
+        }
+        SB_TRY(launch_pyrdown(P.imgs_dev, P.imgs.data(), P.pyr_dev + (size_t)l * n, c->first, c->count, l, mw, mh, s, P.binary_masks));
         SB_TRY(mark("pyrdown_l" + std::to_string(l)));
     }
-    SB_TRY(c->shard.partial_out(c->plan, s));
-    SB_TRY(mark("partial_out"));
     return SB_OK;
 }
 
@@ -619,115 +596,21 @@ static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
     }
     const PanoOut &out = c->slots[slot].out;
     if (!c->sharded) return c->plan.run(out, s, events ? std::function<int(const std::string &)>(mark) : nullptr);
-    if (!c->comm_stream) {
-        SB_CUDA(cudaStreamCreateWithFlags(&c->comm_stream, cudaStreamNonBlocking));
-        for (int k = 0; k < 2; ++k) {
-            SB_CUDA(cudaEventCreateWithFlags(&c->e_part[k], cudaEventDisableTiming));
-            SB_CUDA(cudaEventCreateWithFlags(&c->e_xchg[k], cudaEventDisableTiming));
-        }
+    // sharded: each exchange part is computed and sent in order, then received and finished coarsest first (sb_shard.h)
+    ShardPlan &sh = c->shard;
+    for (int part = 0; part < sh.parts(); ++part) {
+        SB_TRY(shard_local(c, part, s, mark));
+        if (part == 0) SB_TRY(sh.guard(s));
+        SB_TRY(sh.partial_out(c->plan, part, s));
+        SB_TRY(mark(sh.feather ? "partial_out" : part == 0 ? "partial_l0" : "partial_coarse"));
+        SB_TRY(sh.send_part(part, s));
     }
-    BlendPlan &P0 = c->plan;
-    if (P0.kind == SB_BLEND_FEATHER) {
-        // single level: distance-transform weights of the own images, partial sums for the neighbours, one exchange, finish
-        SB_TRY(shard_feather_weights(c, s));
-        SB_TRY(mark("feather_weights"));
-        if (c->shard.connected) {
-            const unsigned step = ++c->shard.step;
-            if (step > 1) SB_CUDA(cudaStreamWaitEvent(s, c->e_xchg[1], 0));  // the previous step's copies have left the send buffers
-            SB_TRY(c->shard.feather_partial_out(P0, s));
-            SB_TRY(mark("partial_out"));
-            SB_CUDA(cudaEventRecord(c->e_part[0], s));
-            SB_CUDA(cudaStreamWaitEvent(c->comm_stream, c->e_part[0], 0));
-            SB_TRY(c->shard.wait_consumed(c->comm_stream, step - 1));
-            SB_TRY(c->shard.push(c->comm_stream, 0));
-            SB_TRY(c->shard.signal_data(c->comm_stream, 0, step));
-            SB_CUDA(cudaEventRecord(c->e_xchg[1], c->comm_stream));
-            SB_TRY(c->shard.wait_data(s, 0, step));
-            SB_TRY(c->shard.feather_finish(P0, out, s));
-            SB_TRY(c->shard.signal_consumed(s, step));
-        } else {
-            SB_TRY(c->shard.feather_partial_out(P0, s));
-            SB_TRY(mark("partial_out"));
-            SB_CUDA(cudaEventRecord(c->e_part[0], s));
-            SB_CUDA(cudaStreamWaitEvent(c->comm_stream, c->e_part[0], 0));
-            SB_TRY(c->shard.exchange(c->comm_stream, -1));
-            SB_CUDA(cudaEventRecord(c->e_xchg[0], c->comm_stream));
-            SB_CUDA(cudaStreamWaitEvent(s, c->e_xchg[0], 0));
-            SB_TRY(c->shard.feather_finish(P0, out, s));
-        }
-        SB_TRY(mark("feather_finish"));
-        return SB_OK;
+    for (int part = sh.parts() - 1; part >= 0; --part) {
+        SB_TRY(sh.receive_part(part, s));
+        SB_TRY(sh.finish(c->plan, out, part, s));
+        if (part == 0) SB_TRY(sh.consumed(s));
+        SB_TRY(mark(sh.feather ? "feather_finish" : part == 0 ? "finish_l0" : "finish_coarse"));  // includes waiting for the slabs
     }
-    if (c->shard.connected) {
-        // Exchange over mapped peer memory (sb_peer.cpp): the slabs go from the local send buffers into the owners' arenas
-        // with copy-engine copies on the communication stream, beside the pyramid kernels; flags written / awaited by
-        // stream memory operations order the ranks (no host round trip, no NCCL call in the step).
-        const unsigned step = ++c->shard.step;
-        const bool direct = c->shard.direct_stores;
-        cudaStream_t cs = direct ? s : c->comm_stream;
-        SB_TRY(shard_pyrdown(c, s, 0));
-        SB_TRY(mark("pyrdown_l0"));
-        if (step > 1 && !direct) SB_CUDA(cudaStreamWaitEvent(s, c->e_xchg[1], 0));  // the previous step's copies have left the send buffers
-        if (direct) SB_TRY(c->shard.wait_consumed(s, step - 1));
-        SB_TRY(c->shard.partial_out(P0, s, 0, 0, direct));
-        SB_TRY(mark("partial_l0"));
-        if (!direct) {
-            SB_CUDA(cudaEventRecord(c->e_part[0], s));
-            SB_CUDA(cudaStreamWaitEvent(cs, c->e_part[0], 0));
-            SB_TRY(c->shard.wait_consumed(cs, step - 1));  // the neighbours have read what the previous step delivered
-            SB_TRY(c->shard.push(cs, 0));
-        }
-        SB_TRY(c->shard.signal_data(cs, 0, step));
-        for (int l = 1; l < P0.nb; ++l) {
-            SB_TRY(shard_pyrdown(c, s, l));
-            SB_TRY(mark("pyrdown_l" + std::to_string(l)));
-        }
-        SB_TRY(c->shard.partial_out(P0, s, 1, P0.nb, direct));
-        SB_TRY(mark("partial_coarse"));
-        if (!direct) {
-            SB_CUDA(cudaEventRecord(c->e_part[1], s));
-            SB_CUDA(cudaStreamWaitEvent(cs, c->e_part[1], 0));
-            SB_TRY(c->shard.push(cs, 1));
-        }
-        SB_TRY(c->shard.signal_data(cs, 1, step));
-        if (!direct) SB_CUDA(cudaEventRecord(c->e_xchg[1], cs));
-        SB_TRY(c->shard.wait_data(s, 1, step));
-        SB_TRY(c->shard.finish(P0, out, s, P0.nb, 1));
-        SB_TRY(mark("finish_coarse"));  // includes waiting for the coarse slabs of the neighbours
-        SB_TRY(c->shard.wait_data(s, 0, step));
-        SB_TRY(c->shard.finish(P0, out, s, 0, 0));
-        SB_TRY(c->shard.signal_consumed(s, step));
-        SB_TRY(mark("finish_l0"));      // includes waiting for the level-0 slabs
-        return SB_OK;
-    }
-    // The exchange overlaps the kernels.  Level 0 of the partial sums -- three quarters of the bytes -- needs only the
-    // first pyrDown, and the collapse reads it last: its slabs travel on the communication stream while the rest of the
-    // pyramid, the coarser partial sums, their (small) exchange and the collapse of levels nb..1 run.
-    BlendPlan &P = c->plan;
-    SB_TRY(shard_pyrdown(c, s, 0));
-    SB_TRY(mark("pyrdown_l0"));
-    SB_TRY(c->shard.partial_out(P, s, 0, 0));
-    SB_TRY(mark("partial_l0"));
-    SB_CUDA(cudaEventRecord(c->e_part[0], s));
-    SB_CUDA(cudaStreamWaitEvent(c->comm_stream, c->e_part[0], 0));
-    SB_TRY(c->shard.exchange(c->comm_stream, 0));
-    SB_CUDA(cudaEventRecord(c->e_xchg[0], c->comm_stream));
-    for (int l = 1; l < P.nb; ++l) {
-        SB_TRY(shard_pyrdown(c, s, l));
-        SB_TRY(mark("pyrdown_l" + std::to_string(l)));
-    }
-    SB_TRY(c->shard.partial_out(P, s, 1, P.nb));
-    SB_TRY(mark("partial_coarse"));
-    SB_CUDA(cudaEventRecord(c->e_part[1], s));
-    SB_CUDA(cudaStreamWaitEvent(c->comm_stream, c->e_part[1], 0));
-    SB_TRY(c->shard.exchange(c->comm_stream, 1));
-    SB_CUDA(cudaEventRecord(c->e_xchg[1], c->comm_stream));
-    SB_CUDA(cudaStreamWaitEvent(s, c->e_xchg[1], 0));
-    SB_TRY(c->shard.finish(P, out, s, P.nb, 1));
-    SB_TRY(mark("finish_coarse"));  // includes waiting for the coarse slabs of the neighbours
-    SB_CUDA(cudaStreamWaitEvent(s, c->e_xchg[0], 0));
-    SB_TRY(c->shard.finish(P, out, s, 0, 0));
-    SB_TRY(mark("finish_l0"));      // includes waiting for the level-0 slabs
     return SB_OK;
 }
 
@@ -872,7 +755,8 @@ int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_lo
 }
 
 // Transport hooks: run the two halves of a sharded step separately and reach the slab buffers, so that a caller can
-// move the slabs itself (tests do, with plain copies; sb_compositor_run uses NCCL).
+// move the slabs itself (tests do, with plain copies; sb_compositor_run uses the transport of ShardPlan).  Phase 0 is the
+// warp and every exchange part's local work and partial sums; phase 1 finishes every part, coarsest first.
 int sb_compositor_shard_phase(sb_compositor *c, int phase)
 {
     if (refuse_timelapse(c, "sb_compositor_shard_phase")) return SB_ERR_STATE;
@@ -881,14 +765,15 @@ int sb_compositor_shard_phase(sb_compositor *c, int phase)
         return SB_ERR_INVALID;
     }
     cudaStream_t s = c->stream;
-    auto nomark = [](const std::string &) -> int { return SB_OK; };
+    ShardPlan &sh = c->shard;
     if (phase == 0) {
         SB_TRY(launch_warp(warp_jobs(c, 0), (int)c->warped.size(), s));
-        SB_TRY(shard_local(c, s, std::function<int(const std::string &)>(nomark)));
-    } else if (c->plan.kind == SB_BLEND_FEATHER) {
-        SB_TRY(c->shard.feather_finish(c->plan, c->slots[0].out, s));
+        for (int part = 0; part < sh.parts(); ++part) {
+            SB_TRY(shard_local(c, part, s, [](const std::string &) -> int { return SB_OK; }));
+            SB_TRY(sh.partial_out(c->plan, part, s));
+        }
     } else {
-        SB_TRY(c->shard.finish(c->plan, c->slots[0].out, s));
+        for (int part = sh.parts() - 1; part >= 0; --part) SB_TRY(sh.finish(c->plan, c->slots[0].out, part, s));
     }
     SB_CUDA(cudaStreamSynchronize(s));
     return SB_OK;

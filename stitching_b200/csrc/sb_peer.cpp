@@ -1,5 +1,5 @@
-// sb_peer.cpp -- the slab exchange of the sharded composite as direct NVLink stores (no reference counterpart: the
-// reference is single-process; this is SURVEY.md 8(e)).
+// sb_peer.cpp -- the transport of the sharded composite's slabs: direct NVLink copies or stores, or the NCCL exchange
+// (no reference counterpart: the reference is single-process; this is SURVEY.md 8(e)).
 //
 // Round 1 moved the slabs with grouped ncclSend / ncclRecv on a communication stream: at 8 GPUs the exchange ran far
 // below link rate and the collapse waited for it (VERDICT r1, item 8).  Here every rank keeps the slabs it RECEIVES
@@ -7,15 +7,17 @@
 // (k_collapse_fast with `partial` set) write their slabs into local send buffers and the copy engines move them into
 // the owners' arenas (cudaMemcpyAsync on the mapped peer pointers: NVLink DMA at link rate, no SM, no NCCL kernel, on
 // a second stream beside the pyramid kernels).  Storing the slabs from the kernels straight into the peers' arenas is
-// available too (SB_PEER=direct) -- it lost where it was measured: the 2- and 4-byte scattered stores of that kernel
-// cross NVLink as small partial writes.  The ranks order themselves with four flags per pair, written by
+// available too (SB_PEER=direct, multiband) -- it lost where it was measured: the 2- and 4-byte scattered stores of
+// that kernel cross NVLink as small partial writes.  The ranks order themselves with flags written by
 // stream memory operations (cuStreamWriteValue32: stream-ordered behind the copy, no host round trip) and awaited by a
 // one-warp polling kernel (k_wait_flags, sb_util.cu) right before the kernel that reads the slab -- cuStreamWaitValue32
 // was measured too and lost: enqueued ahead, the front end evaluates those waits in batches:
-//   data[part][p]  in the RECEIVER's arena: rank p has finished writing part `part` (0: level 0, 1: the coarser
-//                  levels) of step `value`;
+//   data[part][p]  in the RECEIVER's arena: rank p has finished writing exchange part `part` (sb_shard.h) of step
+//                  `value`;
 //   consumed[p]    in the SENDER's arena: rank p has read the slabs of step `value` (the next step may overwrite them).
 // NCCL stays the bootstrap (all-gather of the IPC handles) and the fallback (SB_PEER=0, or a failing connect()).
+// send_part / receive_part at the end of this file hide which of the three moves a part: the step calls them the same way
+// for every blender and transport.
 #include <cstring>
 
 #include "sb_shard.h"
@@ -65,9 +67,8 @@ bool load_memops()
 
 int ShardPlan::connect(const BlendPlan &plan, cudaStream_t s)
 {
-    connected = false;
+    connected = direct_stores = false;
     const char *e = getenv("SB_PEER");
-    direct_stores = e && !strcmp(e, "direct");
     if ((e && e[0] == '0') || !comm_ready() || comm_world() != world || comm_rank() != rank) return SB_OK;  // NCCL exchange
     if (!load_memops()) return SB_OK;
     // my arena: the slabs I receive (they replace the per-peer receive buffers) + the flags
@@ -115,6 +116,7 @@ int ShardPlan::connect(const BlendPlan &plan, cudaStream_t s)
     // the receive slabs now live in the arena (the item lists are built from recv[p].buf afterwards, in allocate())
     recv_off = off;
     connected = true;
+    direct_stores = !feather && e && !strcmp(e, "direct");  // the feather partial sums always go through the send buffers
     step = 0;
     return SB_OK;
 }
@@ -129,12 +131,13 @@ static int memop(MemOpFn fn, cudaStream_t s, void *addr, unsigned value, unsigne
     return SB_OK;
 }
 
-int ShardPlan::push(cudaStream_t s, int part)
+int ShardPlan::push(int part, cudaStream_t s)
 {
     for (int p = 0; p < world; ++p) {
         if (p == rank || !send[p].bytes || !peer_arena[p]) continue;
-        const size_t s0 = part == 1 ? send[p].split : 0, s1 = part == 0 ? send[p].split : send[p].bytes;  // level 0 lies in front
-        if (s1 <= s0) continue;
+        size_t s0, s1;
+        send[p].part_range(part, &s0, &s1);
+        if (s1 == s0) continue;
         SB_CUDA(cudaMemcpyAsync(peer_arena[p] + peer_slot[p] + s0, (const char *)send[p].buf + s0, s1 - s0, cudaMemcpyDeviceToDevice, s));
     }
     return SB_OK;
@@ -180,11 +183,45 @@ int ShardPlan::wait_consumed(cudaStream_t s, unsigned value)
 }
 #else
 int ShardPlan::connect(const BlendPlan &, cudaStream_t) { return SB_OK; }
-int ShardPlan::push(cudaStream_t, int) { return SB_ERR_STATE; }
+int ShardPlan::push(int, cudaStream_t) { return SB_ERR_STATE; }
 int ShardPlan::signal_data(cudaStream_t, int, unsigned) { return SB_ERR_STATE; }
 int ShardPlan::wait_data(cudaStream_t, int, unsigned) { return SB_ERR_STATE; }
 int ShardPlan::signal_consumed(cudaStream_t, unsigned) { return SB_ERR_STATE; }
 int ShardPlan::wait_consumed(cudaStream_t, unsigned) { return SB_ERR_STATE; }
 #endif
+
+int ShardPlan::guard(cudaStream_t s)
+{
+    ++step;
+    if (direct_stores) return wait_consumed(s, step - 1);
+    if (connected && step > 1) SB_CUDA(cudaStreamWaitEvent(s, e_xchg_[parts() - 1], 0));  // the last step's copies have left
+    return SB_OK;
+}
+
+int ShardPlan::send_part(int part, cudaStream_t s)
+{
+    if (direct_stores) return signal_data(s, part, step);  // the partial sums are in the owners' arenas already
+    SB_CUDA(cudaEventRecord(e_part_[part], s));
+    SB_CUDA(cudaStreamWaitEvent(comm_, e_part_[part], 0));
+    if (!connected) {
+        SB_TRY(exchange(part, comm_));
+        SB_CUDA(cudaEventRecord(e_xchg_[part], comm_));
+        return SB_OK;
+    }
+    if (part == 0) SB_TRY(wait_consumed(comm_, step - 1));  // the neighbours have read what the last step delivered
+    SB_TRY(push(part, comm_));
+    SB_TRY(signal_data(comm_, part, step));
+    if (part == parts() - 1) SB_CUDA(cudaEventRecord(e_xchg_[part], comm_));
+    return SB_OK;
+}
+
+int ShardPlan::receive_part(int part, cudaStream_t s)
+{
+    if (connected) return wait_data(s, part, step);
+    SB_CUDA(cudaStreamWaitEvent(s, e_xchg_[part], 0));
+    return SB_OK;
+}
+
+int ShardPlan::consumed(cudaStream_t s) { return connected ? signal_consumed(s, step) : SB_OK; }
 
 }  // namespace sb

@@ -133,10 +133,24 @@ int ShardPlan::build(const BlendPlan &plan, int rank_, int world_)
     }
     rank = rank_;
     world = world_;
+    feather = plan.kind == SB_BLEND_FEATHER;
     axis = 0;
     reversed = false;
     block_of(n, world, rank, &first, &count);
-    if (plan.kind == SB_BLEND_FEATHER) return build_feather(plan);
+    SB_TRY(feather ? feather_bounds(plan) : multiband_bounds(plan));
+    send.assign(world, PeerSlab());
+    recv.assign(world, PeerSlab());
+    for (int p = 0; p < world; ++p) {
+        if (p == rank) continue;
+        slab_geometry(plan, rank, p, &send[p]);
+        slab_geometry(plan, p, rank, &recv[p]);
+    }
+    return SB_OK;
+}
+
+int ShardPlan::multiband_bounds(const BlendPlan &plan)
+{
+    const int n = (int)plan.imgs.size();
     // strip boundaries: halfway between the centres of the neighbouring blocks' edge images, snapped to 2^nb.  Blocks
     // that run right to left would give decreasing boundaries: refused rather than clamped, which would leave one rank
     // the whole panorama and the others nothing.  Equal boundaries (an empty strip) are fine.
@@ -157,19 +171,12 @@ int ShardPlan::build(const BlendPlan &plan, int rank_, int world_)
         }
         bounds[r] = b;
     }
-    send.assign(world, PeerSlab());
-    recv.assign(world, PeerSlab());
-    for (int p = 0; p < world; ++p) {
-        if (p == rank) continue;
-        slab_geometry(plan, rank, p, &send[p]);
-        slab_geometry(plan, p, rank, &recv[p]);
-    }
     return SB_OK;
 }
 
 // Feather: the image blocks are either side by side (a yaw ring: column strips) or stacked (the rows of an affine grid,
 // BASELINE configs[4]: row strips); the strip boundaries lie halfway between the neighbouring blocks' bounding boxes.
-int ShardPlan::build_feather(const BlendPlan &plan)
+int ShardPlan::feather_bounds(const BlendPlan &plan)
 {
     const int n = (int)plan.imgs.size();
     std::vector<double> cx(world), cy(world);
@@ -214,13 +221,6 @@ int ShardPlan::build_feather(const BlendPlan &plan)
         m = std::max(m, bounds[q - 1]);
         bounds[q] = std::min(m, extent);
     }
-    send.assign(world, PeerSlab());
-    recv.assign(world, PeerSlab());
-    for (int p = 0; p < world; ++p) {
-        if (p == rank) continue;
-        slab_geometry(plan, rank, p, &send[p]);
-        slab_geometry(plan, p, rank, &recv[p]);
-    }
     return SB_OK;
 }
 
@@ -236,6 +236,11 @@ int ShardPlan::allocate(const BlendPlan &plan, cudaStream_t s)
 {
     release(s);
     const int n = (int)plan.imgs.size();
+    SB_CUDA(cudaStreamCreateWithFlags(&comm_, cudaStreamNonBlocking));
+    for (int k = 0; k < 2; ++k) {
+        SB_CUDA(cudaEventCreateWithFlags(&e_part_[k], cudaEventDisableTiming));
+        SB_CUDA(cudaEventCreateWithFlags(&e_xchg_[k], cudaEventDisableTiming));
+    }
     SB_TRY(connect(plan, s));  // direct exchange over NVLink when the ranks can map each other's memory (sb_peer.cpp)
     for (int p = 0; p < world; ++p) {
         if (send[p].bytes) SB_TRY(dev_alloc(&send[p].buf, send[p].bytes, s));
@@ -245,7 +250,7 @@ int ShardPlan::allocate(const BlendPlan &plan, cudaStream_t s)
         else
             SB_TRY(dev_alloc(&recv[p].buf, recv[p].bytes, s));
     }
-    if (plan.kind == SB_BLEND_FEATHER) {
+    if (feather) {
         // the slabs this rank receives, lower ranks first
         std::vector<FeatherSlab> fs;
         feather_before_ = feather_after_ = 0;
@@ -321,6 +326,7 @@ int ShardPlan::allocate(const BlendPlan &plan, cudaStream_t s)
 
 void ShardPlan::release(cudaStream_t s)
 {
+    if (comm_) (void)cudaStreamSynchronize(comm_);  // nothing queued there may still use the slabs
     for (auto &p : send) {
         dev_free(p.buf, s);
         p.buf = nullptr;
@@ -338,7 +344,7 @@ void ShardPlan::release(cudaStream_t s)
 #endif
         peer_arena.clear();
         arena = nullptr;
-        connected = false;
+        connected = direct_stores = false;
     }
     dev_free(items_arena_, s);
     items_arena_ = nullptr;
@@ -347,109 +353,102 @@ void ShardPlan::release(cudaStream_t s)
     for (auto &t : tile_items_dev) t = nullptr;
     dev_free(feather_items_, s);
     feather_items_ = nullptr;
-}
-
-int ShardPlan::feather_partial_out(const BlendPlan &plan, cudaStream_t s, bool direct)
-{
-    direct = direct && connected;
-    for (int p = 0; p < world; ++p) {
-        const SlabLevel &L = send[p].lv[0];
-        if (p == rank || !send[p].bytes || L.w == 0) continue;
-        FeatherRegionArgs A;
-        std::memset(&A, 0, sizeof A);
-        A.imgs = plan.imgs_dev;
-        A.i0 = first;
-        A.i1 = first + count;
-        A.rx0 = L.x0; A.ry0 = L.y0; A.rw = L.w; A.rh = L.h;
-        A.partial = 1;
-        char *dst = direct ? peer_arena[p] + peer_slot[p] : (char *)send[p].buf;
-        A.slab_acc = (int16_t *)(dst + L.acc_off);
-        A.slab_w = (float *)(dst + L.w_off);
-        A.slab_pitch = L.pitch;
-        A.slab_plane = L.plane;
-        SB_TRY(launch_feather_region(A, s));
+    if (comm_) (void)cudaStreamDestroy(comm_);
+    comm_ = nullptr;
+    for (int k = 0; k < 2; ++k) {
+        if (e_part_[k]) (void)cudaEventDestroy(e_part_[k]);
+        if (e_xchg_[k]) (void)cudaEventDestroy(e_xchg_[k]);
+        e_part_[k] = e_xchg_[k] = nullptr;
     }
-    return SB_OK;
 }
 
-int ShardPlan::feather_finish(const BlendPlan &plan, const PanoOut &out, cudaStream_t s)
+int ShardPlan::partial_out(const BlendPlan &plan, int part, cudaStream_t s)
 {
-    int lo, hi;
-    strip(plan, &lo, &hi);
-    FeatherRegionArgs A;
-    std::memset(&A, 0, sizeof A);
-    A.imgs = plan.imgs_dev;
-    A.i0 = first;
-    A.i1 = first + count;
-    A.slabs = (const FeatherSlab *)feather_items_;
-    A.n_before = feather_before_;
-    A.n_after = feather_after_;
-    A.rx0 = axis == 0 ? lo : 0;
-    A.ry0 = axis == 0 ? 0 : lo;
-    A.rw = axis == 0 ? hi - lo : plan.roi.w;
-    A.rh = axis == 0 ? plan.roi.h : hi - lo;
-    A.out = out;
-    A.out_x0 = A.rx0;
-    A.out_y0 = A.ry0;
-    return launch_feather_region(A, s);
-}
-
-int ShardPlan::partial_out(const BlendPlan &plan, cudaStream_t s, int l_lo, int l_hi, bool direct)
-{
-    direct = direct && connected;
     const int n = (int)plan.imgs.size();
+    const int l_lo = part, l_hi = part == 0 ? 0 : plan.nb;  // the part's levels
     for (int p = 0; p < world; ++p) {
         if (p == rank || !send[p].bytes) continue;
-        for (int l = std::max(l_lo, 0); l <= std::min(l_hi, plan.nb); ++l) {
+        // direct stores: the slab goes straight to its place in the owner's arena (peer stores over NVLink)
+        char *dst = direct_stores ? peer_arena[p] + peer_slot[p] : (char *)send[p].buf;
+        for (int l = l_lo; l <= l_hi; ++l) {
             const SlabLevel &L = send[p].lv[l];
             if (L.w == 0) continue;
-            CollapseArgs A;
-            std::memset(&A, 0, sizeof A);
-            A.col = plan.col_dev + (size_t)l * n + first;  // this rank's images, contiguous in the level's array
-            A.n = count;
-            A.rx0 = L.x0;
-            A.ry0 = L.y0;
-            A.rw = L.w;
-            A.rh = L.h;
-            A.partial = 1;
-            // direct: the slab is stored straight into its place in the owner's arena (peer stores over NVLink)
-            char *dst = direct ? peer_arena[p] + peer_slot[p] : (char *)send[p].buf;
-            A.slab_acc = (int16_t *)(dst + L.acc_off);
-            A.slab_w = (float *)(dst + L.w_off);
-            A.slab_pitch = L.pitch;
-            A.slab_plane = L.plane;
-            SB_TRY(launch_collapse_fast(A, l, plan.nb, s));
+            auto slab = [&](auto &A) {
+                std::memset(&A, 0, sizeof A);
+                A.rx0 = L.x0;
+                A.ry0 = L.y0;
+                A.rw = L.w;
+                A.rh = L.h;
+                A.partial = 1;
+                A.slab_acc = (int16_t *)(dst + L.acc_off);
+                A.slab_w = (float *)(dst + L.w_off);
+                A.slab_pitch = L.pitch;
+                A.slab_plane = L.plane;
+            };
+            if (feather) {
+                FeatherRegionArgs A;
+                slab(A);
+                A.imgs = plan.imgs_dev;
+                A.i0 = first;
+                A.i1 = first + count;
+                SB_TRY(launch_feather_region(A, s));
+            } else {
+                CollapseArgs A;
+                slab(A);
+                A.col = plan.col_dev + (size_t)l * n + first;  // this rank's images, contiguous in the level's array
+                A.n = count;
+                SB_TRY(launch_collapse_fast(A, l, plan.nb, s));
+            }
         }
     }
     return SB_OK;
 }
 
-int ShardPlan::exchange(cudaStream_t s, int part)
+int ShardPlan::exchange(int part, cudaStream_t s)
 {
     std::vector<int> peers;
     std::vector<void *> sp, rp;
     std::vector<size_t> sb_, rb;
     for (int p = 0; p < world; ++p) {
         if (p == rank || (!send[p].bytes && !recv[p].bytes)) continue;
-        // byte range of the part: level 0 lies in front
-        const size_t s0 = part == 1 ? send[p].split : 0, s1 = part == 0 ? send[p].split : send[p].bytes;
-        const size_t r0 = part == 1 ? recv[p].split : 0, r1 = part == 0 ? recv[p].split : recv[p].bytes;
-        if (s1 <= s0 && r1 <= r0) continue;
+        size_t s0, s1, r0, r1;
+        send[p].part_range(part, &s0, &s1);
+        recv[p].part_range(part, &r0, &r1);
+        if (s1 == s0 && r1 == r0) continue;
         peers.push_back(p);
         sp.push_back((char *)send[p].buf + s0);
-        sb_.push_back(s1 > s0 ? s1 - s0 : 0);
+        sb_.push_back(s1 - s0);
         rp.push_back((char *)recv[p].buf + r0);
-        rb.push_back(r1 > r0 ? r1 - r0 : 0);
+        rb.push_back(r1 - r0);
     }
     if (peers.empty()) return SB_OK;
     return comm_exchange((int)peers.size(), peers.data(), sp.data(), sb_.data(), rp.data(), rb.data(), s);
 }
 
-int ShardPlan::finish(const BlendPlan &plan, const PanoOut &out, cudaStream_t s, int l_hi, int l_lo)
+int ShardPlan::finish(const BlendPlan &plan, const PanoOut &out, int part, cudaStream_t s)
 {
     int lo, hi;
     strip(plan, &lo, &hi);
-    for (int l = std::min(l_hi, plan.nb); l >= std::max(l_lo, 0); --l) {
+    if (feather) {
+        FeatherRegionArgs A;
+        std::memset(&A, 0, sizeof A);
+        A.imgs = plan.imgs_dev;
+        A.i0 = first;
+        A.i1 = first + count;
+        A.slabs = (const FeatherSlab *)feather_items_;
+        A.n_before = feather_before_;
+        A.n_after = feather_after_;
+        A.rx0 = axis == 0 ? lo : 0;
+        A.ry0 = axis == 0 ? 0 : lo;
+        A.rw = axis == 0 ? hi - lo : plan.roi.w;
+        A.rh = axis == 0 ? plan.roi.h : hi - lo;
+        A.out = out;
+        A.out_x0 = A.rx0;
+        A.out_y0 = A.ry0;
+        return launch_feather_region(A, s);
+    }
+    const int l_lo = part, l_hi = part == 0 ? 0 : plan.nb;  // the part's levels
+    for (int l = l_hi; l >= l_lo; --l) {
         int a, b;
         region_x(plan, rank, l, &a, &b);
         CollapseArgs A;

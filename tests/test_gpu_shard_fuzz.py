@@ -1,7 +1,7 @@
 """Seeded random sharded rigs (tests/shard_fuzz.py) on the GPU, every strip bit for bit against the oracle summed in the
 ranks' groups: all ranks on one device with the slabs moved by device copies through the transport hooks; the same
-strips under the A/B switches SB_TILE=0 and SB_PD_BIN=0; and, with two or more GPUs, the real exchange (IPC pushes and
-the NCCL fallback) through sb_compositor_run."""
+strips under the A/B switches SB_TILE=0 and SB_PD_BIN=0; and, with two or more GPUs, the real exchange (IPC pushes, direct
+stores and the NCCL fallback) through sb_compositor_run."""
 import os
 
 import pytest
@@ -110,7 +110,7 @@ def gpu_count():
     return test_gpu_sharded.gpu_count()
 
 
-@pytest.mark.parametrize("peer", ["default", "0"])
+@pytest.mark.parametrize("peer", ["default", "0", "direct"])
 def test_shard_fuzz_real_exchange(tmp_path, peer):
     n = gpu_count()
     if n < 2:
