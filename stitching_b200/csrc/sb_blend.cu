@@ -12,8 +12,6 @@
 //   unpadded roi and fuses cv.convertScaleAbs (blender.py:47).
 //
 // feather / no (blender.py:27-28, 34-36 -> cv.detail_FeatherBlender, cv.detail.Blender): single level.
-#include <cstring>
-
 #include "sb_launch.h"
 #include "sb_gather.cuh"
 
@@ -224,32 +222,11 @@ __global__ void k_dt_cols(const FeedImage *__restrict__ imgs, int i, float sharp
 
 }  // namespace
 
-int launch_collapse(const FeedImage *imgs_dev, const FeedImage *imgs_host, const ColDesc *col, int n, const PanoLevel *pano_dev,
-                    const PanoLevel *pano_host, int l, int nb, int lw, int lh, PanoOut out, cudaStream_t s, const TileDesc *tile)
+int launch_collapse_gather(const FeedImage *imgs_dev, int n, const PanoLevel *pano_dev, int l, int nb, int lw, int lh, PanoOut out,
+                           cudaStream_t s)
 {
     int gw = l == 0 ? out.w : lw, gh = l == 0 ? out.h : lh;
     if (gw <= 0 || gh <= 0) return SB_OK;
-    // the fast kernel works on byte-fed images (RGBM level 0, one colour word per pixel above) and needs at least one band
-    bool packed = true;
-    for (int i = 0; i < n; ++i) packed = packed && imgs_host[i].rgbm != nullptr;
-    if (!use_simple_kernels() && nb >= 1 && packed) {
-        CollapseArgs A;
-        std::memset(&A, 0, sizeof A);
-        A.col = col;
-        A.n = n;
-        if (l < nb) A.up = pano_host[l + 1];
-        A.cur = pano_host[l];
-        A.rw = l == 0 ? (out.w + 1) / 2 * 2 : lw;
-        A.rh = l == 0 ? (out.h + 1) / 2 * 2 : lh;
-        A.out = out;
-        A.out_hi = out.w;
-        A.tile = tile;
-        if (tile && l < nb) {  // shared-memory tiles (sb_collapse_tile.cu) where the launch qualifies
-            const int rc = launch_collapse_tile(A, l, nb, s);
-            if (rc != SB_ERR_STATE) return rc;
-        }
-        return launch_collapse_fast(A, l, nb, s);
-    }
     dim3 block(CL_BX, CL_BY), grid(div_up(gw, CL_BX), div_up(gh, CL_BY));
     launch(k_collapse_gather, grid, block, 0, s, imgs_dev, n, pano_dev, l, nb, lw, lh, out);
     return launch_check("k_collapse_gather");

@@ -497,8 +497,10 @@ __global__ void __launch_bounds__(CF_BX *CF_BY, 5) k_collapse_fast(const __grid_
 
 }  // namespace
 
-int launch_collapse_fast(const CollapseArgs &A, int l, int nb, cudaStream_t s)
+int launch_collapse(const CollapseArgs &A, int l, int nb, cudaStream_t s)
 {
+    const int rc = A.tile ? launch_collapse_tile(A, l, nb, s) : SB_ERR_STATE;
+    if (rc != SB_ERR_STATE) return rc;
     if (A.rw <= 0 || A.rh <= 0) return SB_OK;
     if (A.n > SB_MAX_ITEMS) {
         set_error("collapse: %d items exceed SB_MAX_ITEMS=%d", A.n, SB_MAX_ITEMS);

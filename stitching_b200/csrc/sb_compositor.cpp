@@ -546,25 +546,42 @@ static int compositor_enqueue(sb_compositor *c, bool events, int slot = 0)
     return compositor_enqueue_kernels(c, events, slot);
 }
 
-// sharded step, exchange part `part` (sb_shard.h): what its partial sums read, for the own images -- the feather weights,
-// or the pyrDowns to the part's levels
+// The sharded step's two loops (sb_shard.h); `transport` false leaves out guard, send_part, receive_part and consumed (the
+// transport hooks move the slabs themselves).  Loop 0, each exchange part in order: the own images' work its partial sums
+// read (feather weights, or the pyrDowns to the part's levels), the partial sums, the send.
 template <class Mark>
-static int shard_local(sb_compositor *c, int part, cudaStream_t s, const Mark &mark)
+static int shard_send_parts(sb_compositor *c, bool transport, cudaStream_t s, const Mark &mark)
 {
     BlendPlan &P = c->plan;
-    if (P.kind == SB_BLEND_FEATHER) {
-        SB_TRY(launch_feather_weights(P.imgs_dev + c->first, P.imgs.data() + c->first, c->count, P.sharpness, s));
-        return mark("feather_weights");
-    }
-    const int n = (int)P.imgs.size();
-    for (int l = part == 0 ? 0 : 1; l < (part == 0 ? 1 : P.nb); ++l) {
-        int mw = 0, mh = 0;
-        for (int i = c->first; i < c->first + c->count; ++i) {
-            mw = std::max(mw, P.imgs[i].pw >> (l + 1));
-            mh = std::max(mh, P.imgs[i].ph >> (l + 1));
+    ShardPlan &sh = c->shard;
+    for (int part = 0; part < sh.parts(); ++part) {
+        if (sh.feather) {
+            SB_TRY(launch_feather_weights(P.imgs_dev + c->first, P.imgs.data() + c->first, c->count, P.sharpness, s));
+            SB_TRY(mark("feather_weights"));
+        } else {
+            for (int l = part == 0 ? 0 : 1; l < (part == 0 ? 1 : P.nb); ++l) {
+                SB_TRY(P.pyrdown(l, c->first, c->count, s));
+                SB_TRY(mark("pyrdown_l" + std::to_string(l)));
+            }
         }
-        SB_TRY(launch_pyrdown(P.imgs_dev, P.imgs.data(), P.pyr_dev + (size_t)l * n, c->first, c->count, l, mw, mh, s, P.binary_masks));
-        SB_TRY(mark("pyrdown_l" + std::to_string(l)));
+        if (transport && part == 0) SB_TRY(sh.guard(s));
+        SB_TRY(sh.partial_out(P, part, s));
+        SB_TRY(mark(sh.feather ? "partial_out" : part == 0 ? "partial_l0" : "partial_coarse"));
+        if (transport) SB_TRY(sh.send_part(part, s));
+    }
+    return SB_OK;
+}
+
+// loop 1, coarsest part first: the receive and the finish of the own strip into `out`
+template <class Mark>
+static int shard_finish_parts(sb_compositor *c, const PanoOut &out, bool transport, cudaStream_t s, const Mark &mark)
+{
+    ShardPlan &sh = c->shard;
+    for (int part = sh.parts() - 1; part >= 0; --part) {
+        if (transport) SB_TRY(sh.receive_part(part, s));
+        SB_TRY(sh.finish(c->plan, out, part, s));
+        if (transport && part == 0) SB_TRY(sh.consumed(s));
+        SB_TRY(mark(sh.feather ? "feather_finish" : part == 0 ? "finish_l0" : "finish_coarse"));  // includes waiting for the slabs
     }
     return SB_OK;
 }
@@ -596,22 +613,8 @@ static int compositor_enqueue_kernels(sb_compositor *c, bool events, int slot)
     }
     const PanoOut &out = c->slots[slot].out;
     if (!c->sharded) return c->plan.run(out, s, events ? std::function<int(const std::string &)>(mark) : nullptr);
-    // sharded: each exchange part is computed and sent in order, then received and finished coarsest first (sb_shard.h)
-    ShardPlan &sh = c->shard;
-    for (int part = 0; part < sh.parts(); ++part) {
-        SB_TRY(shard_local(c, part, s, mark));
-        if (part == 0) SB_TRY(sh.guard(s));
-        SB_TRY(sh.partial_out(c->plan, part, s));
-        SB_TRY(mark(sh.feather ? "partial_out" : part == 0 ? "partial_l0" : "partial_coarse"));
-        SB_TRY(sh.send_part(part, s));
-    }
-    for (int part = sh.parts() - 1; part >= 0; --part) {
-        SB_TRY(sh.receive_part(part, s));
-        SB_TRY(sh.finish(c->plan, out, part, s));
-        if (part == 0) SB_TRY(sh.consumed(s));
-        SB_TRY(mark(sh.feather ? "feather_finish" : part == 0 ? "finish_l0" : "finish_coarse"));  // includes waiting for the slabs
-    }
-    return SB_OK;
+    SB_TRY(shard_send_parts(c, true, s, mark));
+    return shard_finish_parts(c, out, true, s, mark);
 }
 
 // every slot has its buffers (and a timelapse its frames): the pipelined path may run
@@ -756,7 +759,7 @@ int sb_compositor_shard_info(const sb_compositor *c, int *first_image, int *n_lo
 
 // Transport hooks: run the two halves of a sharded step separately and reach the slab buffers, so that a caller can
 // move the slabs itself (tests do, with plain copies; sb_compositor_run uses the transport of ShardPlan).  Phase 0 is the
-// warp and every exchange part's local work and partial sums; phase 1 finishes every part, coarsest first.
+// warp and the step's loop 0, phase 1 its loop 1, both without the transport calls.
 int sb_compositor_shard_phase(sb_compositor *c, int phase)
 {
     if (refuse_timelapse(c, "sb_compositor_shard_phase")) return SB_ERR_STATE;
@@ -765,15 +768,12 @@ int sb_compositor_shard_phase(sb_compositor *c, int phase)
         return SB_ERR_INVALID;
     }
     cudaStream_t s = c->stream;
-    ShardPlan &sh = c->shard;
+    auto no_mark = [](const std::string &) -> int { return SB_OK; };
     if (phase == 0) {
         SB_TRY(launch_warp(warp_jobs(c, 0), (int)c->warped.size(), s));
-        for (int part = 0; part < sh.parts(); ++part) {
-            SB_TRY(shard_local(c, part, s, [](const std::string &) -> int { return SB_OK; }));
-            SB_TRY(sh.partial_out(c->plan, part, s));
-        }
+        SB_TRY(shard_send_parts(c, false, s, no_mark));
     } else {
-        for (int part = sh.parts() - 1; part >= 0; --part) SB_TRY(sh.finish(c->plan, c->slots[0].out, part, s));
+        SB_TRY(shard_finish_parts(c, c->slots[0].out, false, s, no_mark));
     }
     SB_CUDA(cudaStreamSynchronize(s));
     return SB_OK;

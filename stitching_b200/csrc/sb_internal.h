@@ -205,11 +205,12 @@ struct CollapseArgs {
     const TileDesc *tile;     // tile kernels: items of this level, same order as col (null: not available for this launch)
     int has_slabs;            // some items are slabs of partial sums (ColDesc kind 1): the tile kernels' slab instantiation
 };
-// the shared-memory tile version of the per-level kernel for the plain single-GPU roles; returns SB_ERR_STATE when the launch
-// does not qualify (the caller then uses launch_collapse_fast)
+// the per-level multiband kernel over A's region: the shared-memory tile kernel where A.tile is given and the launch
+// qualifies, else k_collapse_fast (sb_collapse_fast.cu)
+int launch_collapse(const CollapseArgs &A, int l, int nb, cudaStream_t s);
+// the tile kernel alone (sb_collapse_tile.cu); returns SB_ERR_STATE when the launch does not qualify
 int launch_collapse_tile(const CollapseArgs &A, int l, int nb, cudaStream_t s);
 bool collapse_tile_enabled();
-int launch_collapse_fast(const CollapseArgs &A, int l, int nb, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
 // kernel launchers
@@ -239,17 +240,16 @@ int launch_resize_src(const ResizeJob *jobs, int n_jobs, cudaStream_t s);  // on
 int launch_pack_rgbm(const uint8_t *rgb, long long rgb_pitch, const uint8_t *mask, long long mask_pitch, uint32_t *dst,
                      long long dst_pitch, int w, int h, cudaStream_t s);
 // level `l` -> `l+1` of images [first, first+count)
-// `pyr` / `col`: the compact descriptors of level l for the same images (device pointers, `count` / `n` entries)
+// `pyr`: the compact descriptors of level l of all images (device pointer, indexed like imgs_host)
 // binary_masks: the caller guarantees that every mask byte of these images is 0 or 255 (used for l <= 2; sb_pyrdown_fast.cu)
 int launch_pyrdown(const FeedImage *imgs_dev, const FeedImage *imgs_host, const PyrDesc *pyr, int first, int count, int l,
-                   int max_w, int max_h, cudaStream_t s, bool binary_masks = false);
+                   cudaStream_t s, bool binary_masks);
 // SB_KERNELS=simple selects the one-thread-per-pixel gather kernels everywhere (debugging / A-B parity)
 bool use_simple_kernels();
-// multiband: accumulate + normalise + collapse level l (top-down); at l == 0 writes the final outputs
-struct TileDesc;
-int launch_collapse(const FeedImage *imgs_dev, const FeedImage *imgs_host, const ColDesc *col, int n, const PanoLevel *pano_dev,
-                    const PanoLevel *pano_host, int l, int nb, int lw, int lh, PanoOut out, cudaStream_t s,
-                    const TileDesc *tile = nullptr);
+// multiband with the gather kernel (generic int16 feeds, SB_KERNELS=simple, no bands): accumulate + normalise + collapse
+// level l (top-down) of the lw x lh level; at l == 0 writes the final outputs
+int launch_collapse_gather(const FeedImage *imgs_dev, int n, const PanoLevel *pano_dev, int l, int nb, int lw, int lh, PanoOut out,
+                           cudaStream_t s);
 // feather: distance-transform weight maps, then one fused accumulate/normalise pass; NO blender
 // levels T .. nb in one launch (sb_tail.cu); SB_ERR_STATE: not available (emulation build), launch per level instead
 int launch_tail(const FeedImage *imgs_dev, const PanoLevel *pano_dev, int first, int count, int n, int T, int nb, int wp, int hp, const PanoOut &out,

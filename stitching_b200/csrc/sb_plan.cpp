@@ -349,11 +349,50 @@ void BlendPlan::release(cudaStream_t s)
     tail_state_dev = nullptr;
 }
 
+int BlendPlan::pyrdown(int l, int first, int count, cudaStream_t s) const
+{
+    return launch_pyrdown(imgs_dev, imgs.data(), pyr_dev + (size_t)l * imgs.size(), first, count, l, s, binary_masks);
+}
+
+void BlendPlan::region_x(int x0, int x1, int l, int *a, int *b) const
+{
+    *a = std::max(0, (x0 >> l) - 2);  // the margin the pyrUp of the next finer level reads
+    *b = std::min(wp >> l, (x1 >> l) + 2);
+    if (l == 0) {  // nothing finer reads level 0: no margin, and nothing beyond the (even-rounded) roi
+        *a = x0;
+        *b = std::min(x1, (roi.w + 1) / 2 * 2);
+    }
+    if (*b < *a) *b = *a;
+}
+
+CollapseArgs BlendPlan::collapse_args(int l, int x0, int x1, const ColDesc *col, int n, const TileDesc *tile, const PanoOut &out) const
+{
+    CollapseArgs A;
+    std::memset(&A, 0, sizeof A);
+    A.col = col;
+    A.n = n;
+    if (l < nb) A.up = pano[l + 1];
+    A.cur = pano[l];
+    int b;
+    region_x(x0, x1, l, &A.rx0, &b);
+    A.rw = b - A.rx0;
+    A.rh = l == 0 ? (roi.h + 1) / 2 * 2 : hp >> l;
+    A.out = out;
+    A.out_x0 = x0;
+    A.out_lo = std::min(x0, roi.w);  // the strip's own columns of the roi
+    A.out_hi = std::min(x1, roi.w);
+    A.tile = tile;
+    return A;
+}
+
 int BlendPlan::run(const PanoOut &out, cudaStream_t s, const std::function<int(const std::string &)> &mark)
 {
     const int n = (int)imgs.size();
     auto note = [&](const std::string &name) -> int { return mark ? mark(name) : SB_OK; };
     if (kind == SB_BLEND_MULTIBAND) {
+        // the fast collapse needs byte-fed images (RGBM level 0, one colour word per pixel above) and at least one band
+        bool fast = !use_simple_kernels() && nb >= 1;
+        for (const FeedImage &im : imgs) fast = fast && im.rgbm != nullptr;
         int T = tail_from <= nb ? tail_from : nb + 1;  // levels >= T: one launch (sb_tail.cu)
         bool tail_done = false;
         for (int l = 0; l < nb; ++l) {
@@ -368,18 +407,16 @@ int BlendPlan::run(const PanoOut &out, cudaStream_t s, const std::function<int(c
                 if (rc != SB_ERR_STATE) return rc;
                 T = nb + 1;  // not available here: per-level launches
             }
-            int mw = 0, mh = 0;
-            for (const FeedImage &im : imgs) {
-                mw = std::max(mw, im.pw >> (l + 1));
-                mh = std::max(mh, im.ph >> (l + 1));
-            }
-            SB_TRY(launch_pyrdown(imgs_dev, imgs.data(), pyr_dev + (size_t)l * n, 0, n, l, mw, mh, s, binary_masks));
+            SB_TRY(pyrdown(l, 0, n, s));
             SB_TRY(note("pyrdown_l" + std::to_string(l)));
         }
         for (int l = nb; l >= 0; --l) {
             if (tail_done && l >= T) continue;
-            SB_TRY(launch_collapse(imgs_dev, imgs.data(), col_dev + (size_t)l * n, n, pano_dev, pano, l, nb, wp >> l, hp >> l, out, s,
-                                   tile_dev ? tile_dev + (size_t)l * n : nullptr));
+            if (fast)
+                SB_TRY(launch_collapse(collapse_args(l, 0, wp, col_dev + (size_t)l * n, n, tile_dev ? tile_dev + (size_t)l * n : nullptr, out),
+                                       l, nb, s));
+            else
+                SB_TRY(launch_collapse_gather(imgs_dev, n, pano_dev, l, nb, wp >> l, hp >> l, out, s));
             SB_TRY(note("collapse_l" + std::to_string(l)));
         }
     } else {

@@ -44,8 +44,9 @@ public:
     PyrDesc *pyr_dev = nullptr;
     std::vector<ColDesc> col_host;  // host copies (the sharded compositor builds its item lists from them)
     std::vector<PyrDesc> pyr_host;
-    // tile kernels (sb_collapse_tile.cu): per-(level, image) descriptors; null when the plan does not qualify
-    // (generic int16 feeds, a sharded composite): the fast kernels then do the work
+    // tile kernels (sb_collapse_tile.cu): per-(level, image) descriptors; null when the plan does not qualify (generic
+    // int16 feeds: the fast kernels then do the work) and in a sharded plan, whose strips get their own lists of images
+    // and slabs (ShardPlan::tile_items_dev)
     TileDesc *tile_dev = nullptr;   // [(nb+1)][n]
     bool tile_images_ok = false;    // the images with storage on this device qualify for the tile kernels (sb_collapse_tile.cu)
     static TileDesc tile_desc(const FeedImage &im, int l);
@@ -63,6 +64,12 @@ public:
     int allocate(cudaStream_t s);
     // enqueue all blend kernels; `mark` (optional) is called after each launch with its name (timing hooks)
     int run(const PanoOut &out, cudaStream_t s, const std::function<int(const std::string &)> &mark = nullptr);
+    // multiband, pyrDown of level l -> l+1 for images [first, first + count)
+    int pyrdown(int l, int first, int count, cudaStream_t s) const;
+    // multiband, strip [x0, x1) of padded-pano columns (whole pano: [0, wp)): the columns [*a, *b) of level l it collapses,
+    // and that collapse's arguments over n items `col` (`tile`: their tile descriptors, or null) into `out` (from column x0)
+    void region_x(int x0, int x1, int l, int *a, int *b) const;
+    CollapseArgs collapse_args(int l, int x0, int x1, const ColDesc *col, int n, const TileDesc *tile, const PanoOut &out) const;
     // compulsory HBM traffic per launch, in launch order: (name, bytes)
     std::vector<std::pair<std::string, double>> launch_bytes() const;
     void release(cudaStream_t s);

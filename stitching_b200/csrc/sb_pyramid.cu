@@ -3,6 +3,7 @@
 // Replaces the pyrDown chain of MultiBandBlender::feed (createLaplacePyr on the int16 image and the
 // pyrDown loop over the weight map), reached from stitching/blender.py:41.  The padded copy of the image
 // (copyMakeBorder) is never materialised: level 0 is read through index maps (sb_pyramid.cuh).
+#include <algorithm>
 #include <cstdlib>
 
 #include "sb_launch.h"
@@ -33,13 +34,18 @@ int launch_pyrdown_fast(const PyrDesc *pyr, const FeedImage *imgs_host, int coun
                         cudaStream_t s, bool binary_masks);  // sb_pyrdown_fast.cu
 
 int launch_pyrdown(const FeedImage *imgs_dev, const FeedImage *imgs_host, const PyrDesc *pyr, int first, int count, int l,
-                   int max_w, int max_h, cudaStream_t s, bool binary_masks)
+                   cudaStream_t s, bool binary_masks)
 {
-    // max_w / max_h: largest DESTINATION level size among the images of the batch
-    if (count <= 0 || max_w <= 0 || max_h <= 0) return SB_OK;
-    // the fast kernel works on byte-fed images (RGBM level 0, one colour word per pixel above); generic int16 feeds use the gather kernel
+    // max_w / max_h: largest DESTINATION level size among the images of the batch.  The fast kernel works on byte-fed
+    // images (RGBM level 0, one colour word per pixel above); generic int16 feeds use the gather kernel
+    int max_w = 0, max_h = 0;
     bool packed = true;
-    for (int i = first; i < first + count; ++i) packed = packed && imgs_host[i].rgbm != nullptr;
+    for (int i = first; i < first + count; ++i) {
+        max_w = std::max(max_w, imgs_host[i].pw >> (l + 1));
+        max_h = std::max(max_h, imgs_host[i].ph >> (l + 1));
+        packed = packed && imgs_host[i].rgbm != nullptr;
+    }
+    if (count <= 0 || max_w <= 0 || max_h <= 0) return SB_OK;
 #ifdef SB_EMU
     // the emulation plays a warp's 32 lanes with 32 host threads: correct but slow, so the shuffle kernel runs there only
     // on request (tests/test_host_logic.py sets SB_EMU_LANES around a small case); otherwise the gather kernel

@@ -23,18 +23,6 @@ namespace {
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 }
 
-void ShardPlan::region_x(const BlendPlan &plan, int r, int l, int *a, int *b) const
-{
-    const int wl = plan.wp >> l;
-    *a = std::max(0, (bounds[r] >> l) - 2);
-    *b = std::min(wl, (bounds[r + 1] >> l) + 2);
-    if (l == 0) {  // nothing finer reads level 0: no margin, and nothing beyond the (even-rounded) roi
-        *a = bounds[r];
-        *b = std::min(bounds[r + 1], (plan.roi.w + 1) / 2 * 2);
-    }
-    if (*b < *a) *b = *a;
-}
-
 // Feather (single level): rank `src` hands rank `dst` its partial sums over (bounding box of its images) x (dst's strip).
 void ShardPlan::feather_slab_geometry(const BlendPlan &plan, int src, int dst, PeerSlab *ps) const
 {
@@ -101,7 +89,7 @@ void ShardPlan::slab_geometry(const BlendPlan &plan, int src, int dst, PeerSlab 
             fy1 = std::max(fy1, std::min(py1, ((((Y1 - 1) >> l) + 4) + 1) & even));
         }
         int a, b;
-        region_x(plan, dst, l, &a, &b);
+        plan.region_x(bounds[dst], bounds[dst + 1], l, &a, &b);
         const int x0 = std::max(a, fx0), x1 = std::min(b, fx1);
         if (x1 <= x0 || fy1 <= fy0) continue;
         L.x0 = x0;
@@ -397,7 +385,7 @@ int ShardPlan::partial_out(const BlendPlan &plan, int part, cudaStream_t s)
                 slab(A);
                 A.col = plan.col_dev + (size_t)l * n + first;  // this rank's images, contiguous in the level's array
                 A.n = count;
-                SB_TRY(launch_collapse_fast(A, l, plan.nb, s));
+                SB_TRY(launch_collapse(A, l, plan.nb, s));
             }
         }
     }
@@ -427,9 +415,9 @@ int ShardPlan::exchange(int part, cudaStream_t s)
 
 int ShardPlan::finish(const BlendPlan &plan, const PanoOut &out, int part, cudaStream_t s)
 {
-    int lo, hi;
-    strip(plan, &lo, &hi);
     if (feather) {
+        int lo, hi;
+        strip(plan, &lo, &hi);
         FeatherRegionArgs A;
         std::memset(&A, 0, sizeof A);
         A.imgs = plan.imgs_dev;
@@ -449,30 +437,9 @@ int ShardPlan::finish(const BlendPlan &plan, const PanoOut &out, int part, cudaS
     }
     const int l_lo = part, l_hi = part == 0 ? 0 : plan.nb;  // the part's levels
     for (int l = l_hi; l >= l_lo; --l) {
-        int a, b;
-        region_x(plan, rank, l, &a, &b);
-        CollapseArgs A;
-        std::memset(&A, 0, sizeof A);
-        A.col = items_dev[l];
-        A.n = n_items[l];
-        if (l < plan.nb) A.up = plan.pano[l + 1];
-        A.cur = plan.pano[l];
-        A.rx0 = a;
-        A.ry0 = 0;
-        A.rw = b - a;
-        A.rh = l == 0 ? (plan.roi.h + 1) / 2 * 2 : plan.hp >> l;
-        A.out = out;
-        A.out_x0 = bounds[rank];
-        A.out_lo = lo;
-        A.out_hi = hi;
-        A.tile = tile_items_dev[l];
-        A.has_slabs = n_items[l] > count;
-        // levels 0 and 1 on shared-memory tiles when the strip qualifies (slabs are items of their own kind there)
-        const int rc = A.tile ? launch_collapse_tile(A, l, plan.nb, s) : SB_ERR_STATE;
-        if (rc == SB_ERR_STATE)
-            SB_TRY(launch_collapse_fast(A, l, plan.nb, s));
-        else
-            SB_TRY(rc);
+        CollapseArgs A = plan.collapse_args(l, bounds[rank], bounds[rank + 1], items_dev[l], n_items[l], tile_items_dev[l], out);
+        A.has_slabs = n_items[l] > count;  // slabs are items of their own kind in the tile kernels
+        SB_TRY(launch_collapse(A, l, plan.nb, s));
     }
     return SB_OK;
 }

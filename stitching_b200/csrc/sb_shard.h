@@ -91,7 +91,6 @@ public:
     int connect(const BlendPlan &plan, cudaStream_t s);            // collective over the NCCL communicator
 
 private:
-    void region_x(const BlendPlan &plan, int r, int l, int *a, int *b) const;
     void slab_geometry(const BlendPlan &plan, int src, int dst, PeerSlab *ps) const;
     void feather_slab_geometry(const BlendPlan &plan, int src, int dst, PeerSlab *ps) const;
     int multiband_bounds(const BlendPlan &plan);

@@ -3,6 +3,7 @@
 seed_from_env    the seed of a set: its fixed default, an integer or a fresh random draw.
 oracle_image     one image through the Stitcher's FINAL chain on the CPU oracle; oracle_blend: the Blender after it.
 set_extras       a case's per-image extras on a Compositor; compositor_run: one Compositor over a rig_fuzz case.
+device_copy      the slab mover of the transport hooks with every rank on one GPU.
 blend_geometry   the pano roi, blend kind, band count and padded feed rects the library derives from a rig.
 draw_crop        the search for a random largest interior rectangle that leaves every image a non-empty slice.
 ab_run           a function in child processes, with the library's defaults and under each A/B switch.
@@ -89,6 +90,13 @@ def compositor_run(case, imgs, ex, **compositor_kwargs):
                     warped=[w for w, _ in warped], masks=[m for _, m in warped])
     finally:
         c.close()
+
+
+def device_copy(dst, src, nbytes):
+    """copy(dst, src, bytes) for shard_fuzz.hooks_run with all ranks on one GPU: sb_device_copy of a slab."""
+    from stitching_b200 import _lib
+
+    _lib.check(_lib.lib().sb_device_copy(dst, src, nbytes), "sb_device_copy")
 
 
 # -- the blend geometry, restated from the library's plan ---------------------------------------------------------------

@@ -568,15 +568,10 @@ def check(case, got, slab_sizes, ref, seed):
 
 def ab_arrays(seed, ks):
     """Cases `ks` of the GPU set, all ranks on this device: every rank's strip and its mask by name."""
-    from stitching_b200 import _lib
-
-    def copy(d, s, n):
-        _lib.check(_lib.lib().sb_device_copy(d, s, n), "sb_device_copy")
-
     cs = gpu_set(seed)
     out = {}
     for k in ks:
-        got, _ = hooks_run(cs[k], rig_fuzz.images(cs[k]), rig_fuzz.extras(cs[k]), copy)
+        got, _ = hooks_run(cs[k], rig_fuzz.images(cs[k]), rig_fuzz.extras(cs[k]), fuzz_chain.device_copy)
         for r, g in enumerate(got):
             out[f"{k}_{r}_pano"], out[f"{k}_{r}_pmask"] = g["pano"], g["pmask"]
     return out

@@ -1,6 +1,5 @@
 """The compositor with a crop (Stitcher's default Cropper) on the GPU: seeded crops bit for bit against the CPU oracle,
 the full crop against no crop, submit / wait against composite(), the A/B switches, and the sharded roles on one GPU."""
-import ctypes as C
 import os
 
 import numpy as np
@@ -87,12 +86,6 @@ def test_ab_switches_with_a_crop_give_identical_bytes(cuda_lib):
                       [("SB_TILE", "0"), ("SB_PD_BIN", "0"), ("SB_SRC4", "0"), ("SB_GRAPH", "0")], "SB_CROP_FUZZ_SEED")
 
 
-def _device_copy(d, s, n):
-    from stitching_b200 import _lib
-
-    _lib.check(_lib.lib().sb_device_copy(C.c_void_p(d), C.c_void_p(s), n), "sb_device_copy")
-
-
 def test_sharded_crop_roles_on_one_gpu(cuda_lib, oracle):
     """All ranks of a cropped sharded composite on one GPU, the slabs moved with device copies: every strip equals the
     grouped oracle fed with the cropped images."""
@@ -100,7 +93,7 @@ def test_sharded_crop_roles_on_one_gpu(cuda_lib, oracle):
     ran = set()
     for cc in cs:
         for world in (2, 3):
-            if cc.n >= world and crop_fuzz.sharded_check(oracle, cc, world, _device_copy, SEED):
+            if cc.n >= world and crop_fuzz.sharded_check(oracle, cc, world, fuzz_chain.device_copy, SEED):
                 ran.add(world)
     assert ran == {2, 3}, f"worlds run: {sorted(ran)} of {len(cs)} cases"
 

@@ -1,8 +1,6 @@
 """Camera frames resized to FINAL inside the compositor on the GPU: the resize kernel against the oracle, rig / crop /
 shard draws against the compositor fed resized frames, the reference Stitcher's final_megapix records replayed from
 the camera views, SB_SRC4=0 in a child process, and one 48 MP camera."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -12,7 +10,6 @@ import fuzz_chain
 import reference_cases as RC
 import rig_fuzz
 import shard_fuzz
-from stitching_b200 import _lib
 
 pytestmark = pytest.mark.gpu
 
@@ -51,16 +48,12 @@ def test_resized_crop_equals_prefed(cuda_lib, oracle, k):
     final_scale.rig_check(oracle, cc.case, SEED, crop=cc.crop, ex=rig_fuzz.extras(cc.cropped_case()))
 
 
-def _device_copy(d, s, n):
-    _lib.check(_lib.lib().sb_device_copy(C.c_void_p(d), C.c_void_p(s), n), "sb_device_copy")
-
-
 def test_resized_sharded_roles_on_one_gpu(cuda_lib, oracle):
     ran = set()
     for case in shard_fuzz.cases(SEED, 6, rig_fuzz.GPU):
         for world in (2, 3):
             if case.n >= world:
-                final_scale.sharded_check(oracle, case, world, _device_copy, SEED)
+                final_scale.sharded_check(oracle, case, world, fuzz_chain.device_copy, SEED)
                 ran.add(world)
     assert ran == {2, 3}
 

@@ -4,6 +4,7 @@ through ExposureErrorCompensator.apply (host buffers and device twins) and Compo
 import numpy as np
 import pytest
 
+import fuzz_chain
 import gain_maps as GM
 import replay
 from stitching_b200 import exposure_error_compensator as ec
@@ -13,12 +14,6 @@ pytestmark = pytest.mark.gpu
 
 def _apply(img, gain):
     return ec.apply_gain(img, gain)
-
-
-def _device_copy(d, s, n):
-    from stitching_b200 import _lib
-
-    _lib.check(_lib.lib().sb_device_copy(d, s, n), "sb_device_copy")
 
 
 def test_goldens(cuda_lib, oracle):
@@ -48,7 +43,7 @@ def test_timelapse_with_clipped_parts(cuda_lib, oracle):
 
 
 def test_sharded_owner_sets_the_gain(cuda_lib, oracle):
-    GM.check_sharded(oracle, _device_copy, scale_down=4)
+    GM.check_sharded(oracle, fuzz_chain.device_copy, scale_down=4)
 
 
 def test_live_sweep_against_cv2(cuda_lib, oracle):

@@ -10,6 +10,7 @@ import time
 import numpy as np
 import pytest
 
+import fuzz_chain
 import replay
 from stitching_b200 import Blender, Compositor, Warper, rigs
 
@@ -249,13 +250,7 @@ def test_sharded_roles_on_one_gpu(cuda_lib, oracle, name, scale_down, world):
     cams = cfg["cameras"]
     imgs = [rigs.noise_image(cfg["h"], cfg["w"], 70 + i) if i % 2 else rigs.synth_image(cfg["h"], cfg["w"], 70 + i)
             for i in range(len(cams))]
-
-    def copy(dst, src, n):
-        from stitching_b200 import _lib
-
-        _lib.check(cuda_lib.sb_device_copy(dst, src, n), "sb_device_copy")
-
-    pano, mask, moved = test_sharded.run_sharded(cfg, cams, imgs, world, copy)
+    pano, mask, moved = test_sharded.run_sharded(cfg, cams, imgs, world, fuzz_chain.device_copy)
     assert moved > 0
     test_sharded.assert_grouped(oracle, cfg, cams, imgs, world, pano, mask)
     print(f"{name} x{world}: {moved / 1e6:.1f} MB of slabs")

@@ -17,18 +17,12 @@ pytestmark = pytest.mark.gpu
 SEED = shard_fuzz.seed_from_env()
 
 
-def _device_copy(d, s, n):
-    from stitching_b200 import _lib
-
-    _lib.check(_lib.lib().sb_device_copy(d, s, n), "sb_device_copy")
-
-
 @pytest.mark.parametrize("k", range(len(shard_fuzz.gpu_ids())), ids=shard_fuzz.gpu_ids())
 def test_shard_fuzz_on_one_gpu(cuda_lib, oracle, k):
     case = shard_fuzz.gpu_set(SEED)[k]
     imgs, ex = rig_fuzz.images(case), rig_fuzz.extras(case)
     ref = shard_fuzz.grouped_oracle(oracle, case, imgs, ex)
-    got, sizes = shard_fuzz.hooks_run(case, imgs, ex, _device_copy)
+    got, sizes = shard_fuzz.hooks_run(case, imgs, ex, fuzz_chain.device_copy)
     shard_fuzz.check(case, got, sizes, ref, SEED)
 
 

@@ -18,37 +18,18 @@ from stitching_b200 import Compositor, rigs
 
 
 def run_sharded(cfg, cams, imgs, world, copy):
-    sizes = [(cfg["w"], cfg["h"])] * len(cams)
-    ranks = [Compositor(cams, sizes, cfg["warper"], cfg["blender"], cfg["strength"], rank=r, world=world) for r in range(world)]
-    assert sum(c.count for c in ranks) == len(cams) and [c.first for c in ranks] == sorted(c.first for c in ranks)
-    for c in ranks:
-        c.upload(imgs[c.first: c.first + c.count])
-        c.shard_phase(0)
-    moved = 0
-    for src in ranks:
-        for dst in ranks:
-            if src is dst:
-                continue
-            sp, sn = src.shard_slab(dst.rank, True)
-            dp, dn = dst.shard_slab(src.rank, False)
-            assert sn == dn, "both sides must agree on the slab size"
-            if sn:
-                copy(dp, sp, sn)
-                moved += sn
-    strips = []
-    for c in ranks:
-        c.shard_phase(1)
-        strips.append(c.download())
-    axis = ranks[0].strip_axis
-    assert all(c.strip_axis == axis for c in ranks)
-    order = sorted(range(world), key=lambda r: ranks[r].strip)  # spatial order of the strips (feather may run against the rank order)
-    los = [ranks[r].strip for r in order]
-    assert los[0][0] == 0 and all(a[1] == b[0] for a, b in zip(los, los[1:])) and los[-1][1] == ranks[0].roi[3 if axis else 2]
-    pano = np.concatenate([strips[r][0] for r in order], axis=0 if axis else 1)
-    mask = np.concatenate([strips[r][1] for r in order], axis=0 if axis else 1)
-    for c in ranks:
-        c.close()
-    return pano, mask, moved
+    """All ranks of a fixed rig through the transport hooks (shard_fuzz.hooks_run), the slabs moved with `copy`:
+    (panorama, mask, slab bytes moved) of the strips put together."""
+    case = shard_fuzz.config_case(cfg, world, cams)
+    got, sizes = shard_fuzz.hooks_run(case, imgs, [(None, None, None)] * case.n, copy)
+    assert sum(g["count"] for g in got) == len(cams) and [g["first"] for g in got] == sorted(g["first"] for g in got)
+    assert all(sn == dn for sn, dn in sizes.values()), "both sides must agree on the slab size"
+    axis = got[0]["axis"]
+    assert all(g["axis"] == axis for g in got)
+    los = sorted(g["strip"] for g in got)  # spatial order of the strips (feather may run against the rank order)
+    assert los[0][0] == 0 and all(a[1] == b[0] for a, b in zip(los, los[1:])) and los[-1][1] == got[0]["roi"][3 if axis else 2]
+    pano, mask = shard_fuzz.assemble(got)
+    return pano, mask, sum(sn for sn, _ in sizes.values())
 
 
 def assert_grouped(oracle, cfg, cams, imgs, world, pano, mask):
