@@ -1,81 +1,14 @@
-// sb_api.cpp -- the C ABI (include/stitch_b200.h): Warper and Blender entry points with host buffers.
-#include <algorithm>
+// sb_api.cpp -- the C ABI (include/stitch_b200.h): Warper and Blender entry points with host buffers.  Each of them checks
+// its arguments, stages the host buffers on the device, runs the device core and finishes (sb::Staging).
 #include <cstring>
 #include <mutex>
-#include <memory>
 #include <vector>
 
 #include "sb_plan.h"
 
 using namespace sb;
 
-namespace {
-
-bool valid_warp_type(int t) { return t >= SB_WARP_SPHERICAL && t <= SB_WARP_TRANSVERSE_MERCATOR; }
-
-// temp device buffers freed in stream order when the scope ends
-struct Scratch {
-    cudaStream_t s;
-    std::vector<void *> ptrs;
-    explicit Scratch(cudaStream_t st) : s(st) {}
-    ~Scratch()
-    {
-        for (void *p : ptrs) dev_free(p, s);
-    }
-    template <typename T>
-    int get(T **p, size_t count)
-    {
-        void *q = nullptr;
-        int r = dev_alloc(&q, count * sizeof(T), s);
-        if (r == SB_OK) ptrs.push_back(q);
-        *p = (T *)q;
-        return r;
-    }
-};
-
-}  // namespace
-
-namespace sb {
-// shared with the compositor: builds the device tables + job for one image; tables go into `tab` (4 arrays)
-int make_warp_job(const Projector &p, const int rect[4], int src_w, int src_h, float *tab_dev, WarpJob *job, cudaStream_t s,
-                  std::vector<float> &host_tab)
-{
-    const int w = rect[2], h = rect[3];
-    const int wp = (w + 3) & ~3;
-    host_tab.assign(warp_table_floats(w, h), 0.f);
-    float *colX = host_tab.data(), *colZ = colX + wp, *rowA = colZ + wp, *rowY = rowA + h;
-    if (!projector_needs_maps(p)) projector_tables(p, rect, colX, colZ, rowA, rowY);  // (else: warp_maps_upload)
-    SB_CUDA(cudaMemcpyAsync(tab_dev, host_tab.data(), host_tab.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-    std::memset(job, 0, sizeof *job);
-    job->sw = src_w;
-    job->sh = src_h;
-    job->dw = w;
-    job->dh = h;
-    job->colX = tab_dev;
-    job->colZ = tab_dev + wp;
-    job->rowA = tab_dev + 2 * wp;
-    job->rowY = tab_dev + 2 * wp + h;
-    std::memcpy(job->k, p.k_rinv, sizeof job->k);
-    job->always_divide = p.type == SB_WARP_PLANE;
-    job->xmap = job->ymap = nullptr;
-    job->xin_hi = 32.f * (float)(src_w - 1) - 0.5f;
-    job->yin_hi = 32.f * (float)(src_h - 1) - 0.5f;
-    return SB_OK;
-}
-// projections that are not separable: the float maps of buildMaps, built on the host (libm, all cores) and uploaded;
-// `maps_dev` holds xmap then ymap (w * h floats each)
-int warp_maps_upload(const Projector &p, const int rect[4], float *maps_dev, WarpJob *job, cudaStream_t s)
-{
-    const size_t n = (size_t)rect[2] * rect[3];
-    std::vector<float> host(2 * n);
-    projector_maps(p, rect, host.data(), host.data() + n);
-    SB_CUDA(cudaMemcpyAsync(maps_dev, host.data(), 2 * n * sizeof(float), cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaStreamSynchronize(s));  // `host` is a local
-    job->xmap = maps_dev;
-    job->ymap = maps_dev + n;
-    return SB_OK;
-}
-}  // namespace sb
+static bool valid_warp_type(int t) { return t >= SB_WARP_SPHERICAL && t <= SB_WARP_TRANSVERSE_MERCATOR; }
 
 struct sb_devimg {
     uint8_t *p;
@@ -174,51 +107,37 @@ static int warp_impl(int warp_type, float scale, const float K[9], const float R
         return SB_ERR_INVALID;
     }
     SB_TRY(ensure_device());
-    cudaStream_t s = default_stream();
-    Scratch tmp(s);
-    float *tab = nullptr;
-    uint8_t *d_src = nullptr, *d_img = nullptr, *d_mask = nullptr;
-    SB_TRY(tmp.get(&tab, warp_table_floats(w, h)));
     std::vector<float> host_tab;
+    Staging st(default_stream());
+    cudaStream_t s = st.stream();
     WarpJob job;
-    SB_TRY(make_warp_job(p, rect, src_w, src_h, tab, &job, s, host_tab));
+    float *tab = st.tmp<float>(warp_table_floats(w, h));
+    st.run([&] { return make_warp_job(p, rect, src_w, src_h, tab, &job, s, host_tab); });
     if (projector_needs_maps(p)) {
-        float *maps = nullptr;
-        SB_TRY(tmp.get(&maps, (size_t)2 * w * h));
-        SB_TRY(warp_maps_upload(p, rect, maps, &job, s));
+        float *maps = st.tmp<float>((size_t)2 * w * h);
+        st.run([&] { return warp_maps_upload(p, rect, maps, &job, s); });
     }
+    // the kept image and mask survive the call inside their handles
     const bool keep_i = dst_img && keep_img, keep_m = dst_mask && keep_mask;
+    uint8_t *d_img = nullptr, *d_mask = nullptr;
     if (dst_img) {
-        SB_TRY(tmp.get(&d_src, (size_t)src_w * 3 * src_h + SB_SRC_PAD));
-        if (keep_i)
-            SB_TRY(dev_alloc((void **)&d_img, (size_t)w * 3 * h, s));  // survives the call inside the handle
-        else
-            SB_TRY(tmp.get(&d_img, (size_t)w * 3 * h));
-        SB_CUDA(sb_copy2d(d_src, (size_t)src_w * 3, src, src_pitch, (size_t)src_w * 3, src_h, cudaMemcpyHostToDevice, s));
+        uint8_t *d_src = st.tmp<uint8_t>((size_t)src_w * 3 * src_h + SB_SRC_PAD);
+        d_img = keep_i ? st.keep<uint8_t>((size_t)w * 3 * h) : st.tmp<uint8_t>((size_t)w * 3 * h);
+        st.copy(d_src, (size_t)src_w * 3, src, src_pitch, (size_t)src_w * 3, src_h, cudaMemcpyHostToDevice);
         job.src = d_src;
         job.spitch = (long long)src_w * 3;
         job.dst_rgb = d_img;
         job.dst_pitch = (long long)w * 3;
     }
     if (dst_mask) {
-        if (keep_m)
-            SB_TRY(dev_alloc((void **)&d_mask, (size_t)w * h, s));
-        else
-            SB_TRY(tmp.get(&d_mask, (size_t)w * h));
+        d_mask = keep_m ? st.keep<uint8_t>((size_t)w * h) : st.tmp<uint8_t>((size_t)w * h);
         job.dst_mask = d_mask;
         job.mask_pitch = w;
     }
-    int rc = launch_warp(&job, 1, s);
-    if (rc == SB_OK && dst_img && sb_copy2d(dst_img, dst_pitch, d_img, (size_t)w * 3, (size_t)w * 3, h, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-        rc = cuda_fail(cudaGetLastError(), "cudaMemcpy2DAsync", __FILE__, __LINE__);
-    if (rc == SB_OK && dst_mask && sb_copy2d(dst_mask, mask_pitch, d_mask, w, w, h, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-        rc = cuda_fail(cudaGetLastError(), "cudaMemcpy2DAsync", __FILE__, __LINE__);
-    if (cudaStreamSynchronize(s) != cudaSuccess && rc == SB_OK) rc = cuda_fail(cudaGetLastError(), "cudaStreamSynchronize", __FILE__, __LINE__);
-    if (rc != SB_OK) {
-        if (keep_i) dev_free(d_img, s);
-        if (keep_m) dev_free(d_mask, s);
-        return rc;
-    }
+    st.run([&] { return launch_warp(&job, 1, s); });
+    if (dst_img) st.down(dst_img, dst_pitch, d_img, (size_t)w * 3, (size_t)w * 3, h);
+    if (dst_mask) st.down(dst_mask, mask_pitch, d_mask, w, w, h);
+    SB_TRY(st.finish());
     if (keep_i) *keep_img = new sb_devimg{d_img, w, h, 3};
     if (keep_m) *keep_mask = new sb_devimg{d_mask, w, h, 1};
     return SB_OK;
@@ -258,108 +177,26 @@ int sb_devimg_info(const sb_devimg *d, int *w, int *h, int *channels)
 
 }  // extern "C"
 
-namespace sb {
-// SeamFinder.resize on the device: seam mask from the host, `mask_dev` / `dst_dev` on the device (mask_dev may be null)
-int seam_resize_device(const uint8_t *seam_host, size_t seam_pitch, int sw, int sh, const uint8_t *mask_dev, long long mask_pitch,
-                       uint8_t *dst_dev, long long dst_pitch, int w, int h, cudaStream_t s)
-{
-    Scratch tmp(s);
-    uint8_t *d_seam = nullptr, *d_dil = nullptr;
-    int *d_tx = nullptr, *d_ty = nullptr;
-    SB_TRY(tmp.get(&d_seam, (size_t)sw * sh));
-    SB_TRY(tmp.get(&d_dil, (size_t)sw * sh));
-    SB_TRY(tmp.get(&d_tx, (size_t)4 * w));
-    SB_TRY(tmp.get(&d_ty, (size_t)4 * h));
-    std::vector<int> tx((size_t)4 * w), ty((size_t)4 * h);
-    resize_linear_taps(sw, w, true, tx.data());
-    resize_linear_taps(sh, h, false, ty.data());
-    SB_CUDA(sb_copy2d(d_seam, sw, seam_host, seam_pitch, sw, sh, cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaMemcpyAsync(d_tx, tx.data(), tx.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaMemcpyAsync(d_ty, ty.data(), ty.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    SB_TRY(launch_seam_resize(d_seam, sw, sh, d_dil, d_tx, d_ty, mask_dev, mask_pitch, dst_dev, dst_pitch, w, h, s));
-    SB_CUDA(cudaStreamSynchronize(s));  // the tap vectors and the scratch buffers go out of scope
-    return SB_OK;
-}
-}  // namespace sb
-
-namespace sb {
-void gain_free(GainData *gd, cudaStream_t s)
-{
-    dev_free(gd->map, s);
-    dev_free(gd->fx, s);
-    dev_free(gd->fy, s);
-    dev_free(gd->tx, s);
-    dev_free(gd->ty, s);
-    dev_free(gd->lut, s);
-    *gd = GainData{};
-}
-
-// ExposureErrorCompensator.apply's per-image data on the device: either the float32 gain map (gc = 1 or 3 channels) with
-// the resize taps for a w x h image, or the three 256-entry tables of scalar gains
-int gain_upload(WarpJob *job, GainData *gd, int w, int h, const float *gain_map, int gw, int gh, int gc, const double *gain_scalar,
-                cudaStream_t s, const int *sub)
-{
-    gain_free(gd, s);
-    job->gain_mode = 0;
-    if (gain_scalar) {
-        uint8_t lut[768];
-        gain_scalar_lut(gain_scalar, lut);
-        SB_TRY(dev_alloc((void **)&gd->lut, sizeof lut, s));
-        SB_CUDA(cudaMemcpyAsync(gd->lut, lut, sizeof lut, cudaMemcpyHostToDevice, s));
-        SB_CUDA(cudaStreamSynchronize(s));
-        job->gain_lut = gd->lut;
-        job->gain_mode = 2;
-        return SB_OK;
-    }
-    if (!gain_map) return SB_OK;  // no gain: compensator "no"
-    std::vector<int> tx((size_t)2 * w), ty((size_t)2 * h);
-    std::vector<float> fx((size_t)w), fy((size_t)h);
-    // cv::resize runs IPP's kernel on a map with both sides >= 2 and OpenCV's own on a map with a side of 1
-    const bool generic = gw == 1 || gh == 1;
-    resize_f32_taps(gw, w, tx.data(), fx.data(), generic ? TAPS_COLS : TAPS_IPP);
-    resize_f32_taps(gh, h, ty.data(), fy.data(), generic ? TAPS_ROWS : TAPS_IPP);
-    if (sub) {
-        // the taps of columns [x, x + w') and rows [y, y + h') of the whole image: [i0 | i1] halves cut alike
-        auto cut = [](std::vector<int> &t, std::vector<float> &f, int n, int o, int m) {
-            std::vector<int> t2((size_t)2 * m);
-            for (int k = 0; k < m; ++k) {
-                t2[k] = t[o + k];
-                t2[m + k] = t[n + o + k];
-            }
-            t.swap(t2);
-            f = std::vector<float>(f.begin() + o, f.begin() + o + m);
-        };
-        cut(tx, fx, w, sub[0], sub[2]);
-        cut(ty, fy, h, sub[1], sub[3]);
-    }
-    SB_TRY(dev_alloc((void **)&gd->map, sizeof(float) * (size_t)gw * gh * gc, s));
-    SB_TRY(dev_alloc((void **)&gd->tx, sizeof(int) * tx.size(), s));
-    SB_TRY(dev_alloc((void **)&gd->ty, sizeof(int) * ty.size(), s));
-    SB_TRY(dev_alloc((void **)&gd->fx, sizeof(float) * fx.size(), s));
-    SB_TRY(dev_alloc((void **)&gd->fy, sizeof(float) * fy.size(), s));
-    SB_CUDA(cudaMemcpyAsync(gd->map, gain_map, sizeof(float) * (size_t)gw * gh * gc, cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaMemcpyAsync(gd->tx, tx.data(), sizeof(int) * tx.size(), cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaMemcpyAsync(gd->ty, ty.data(), sizeof(int) * ty.size(), cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaMemcpyAsync(gd->fx, fx.data(), sizeof(float) * fx.size(), cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaMemcpyAsync(gd->fy, fy.data(), sizeof(float) * fy.size(), cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaStreamSynchronize(s));
-    job->gain_map = gd->map;
-    job->gain_tx = gd->tx;
-    job->gain_ty = gd->ty;
-    job->gain_fx = gd->fx;
-    job->gain_fy = gd->fy;
-    job->gain_gw = gw;
-    job->gain_gc = gc;
-    job->gain_mode = generic ? 3 : 1;
-    return SB_OK;
-}
-}  // namespace sb
-
 static bool valid_gain_args(const float *gain_map, int gw, int gh, int gc, const double *gain_scalar)
 {
     if (gain_map && gain_scalar) return false;
     if (gain_map && (gw <= 0 || gh <= 0 || (gc != 1 && gc != 3))) return false;
     return true;
+}
+
+// ExposureErrorCompensator.apply on a device rectangle (pitch in bytes), then its copy to `host` when one is given
+static int gain_apply(Staging &st, uint8_t *img, long long pitch, int w, int h, uint8_t *host, size_t host_pitch, const float *gain_map,
+                      int gw, int gh, int gc, const double *gain_scalar)
+{
+    WarpJob job;
+    std::memset(&job, 0, sizeof job);
+    GainData gd;
+    st.run([&] { return gain_upload(&job, &gd, w, h, gain_map, gw, gh, gc, gain_scalar, st.stream()); });
+    st.run([&] { return launch_gain_apply(img, pitch, w, h, job, st.stream()); });
+    if (host) st.down(host, host_pitch, img, (size_t)pitch, (size_t)w * 3, h);
+    const int rc = st.finish();
+    gain_free(&gd, st.stream());
+    return rc;
 }
 
 extern "C" {
@@ -372,21 +209,9 @@ int sb_gain_apply(uint8_t *img, size_t pitch, int w, int h, const float *gain_ma
     }
     if (!gain_map && !gain_scalar) return SB_OK;  // compensator "no": identity
     SB_TRY(ensure_device());
-    cudaStream_t s = default_stream();
-    Scratch tmp(s);
-    uint8_t *d_img = nullptr;
-    SB_TRY(tmp.get(&d_img, (size_t)w * 3 * h));
-    SB_CUDA(sb_copy2d(d_img, (size_t)w * 3, img, pitch, (size_t)w * 3, h, cudaMemcpyHostToDevice, s));
-    WarpJob job;
-    std::memset(&job, 0, sizeof job);
-    GainData gd;
-    int rc = gain_upload(&job, &gd, w, h, gain_map, gw, gh, gc, gain_scalar, s);
-    if (rc == SB_OK) rc = launch_gain_apply(d_img, (long long)w * 3, w, h, job, s);
-    if (rc == SB_OK && sb_copy2d(img, pitch, d_img, (size_t)w * 3, (size_t)w * 3, h, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-        rc = SB_ERR_CUDA;
-    if (cudaStreamSynchronize(s) != cudaSuccess && rc == SB_OK) rc = SB_ERR_CUDA;
-    gain_free(&gd, s);
-    return rc;
+    Staging st(default_stream());
+    uint8_t *d_img = st.up<uint8_t>(img, pitch, (size_t)w * 3, h);
+    return gain_apply(st, d_img, (long long)w * 3, w, h, img, pitch, gain_map, gw, gh, gc, gain_scalar);
 }
 
 int sb_gain_apply_dev(sb_devimg *img, int x, int y, int w, int h, uint8_t *host, size_t host_pitch, const float *gain_map, int gw, int gh,
@@ -399,20 +224,9 @@ int sb_gain_apply_dev(sb_devimg *img, int x, int y, int w, int h, uint8_t *host,
     }
     if (!gain_map && !gain_scalar) return SB_OK;  // compensator "no": identity (host and device copies stay as they are)
     SB_TRY(ensure_device());
-    cudaStream_t s = default_stream();
+    Staging st(default_stream());
     uint8_t *view = img->p + ((size_t)y * img->w + x) * 3;
-    const long long pitch = (long long)img->w * 3;
-    WarpJob job;
-    std::memset(&job, 0, sizeof job);
-    GainData gd;
-    int rc = gain_upload(&job, &gd, w, h, gain_map, gw, gh, gc, gain_scalar, s);
-    if (rc == SB_OK) rc = launch_gain_apply(view, pitch, w, h, job, s);
-    if (rc == SB_OK && host && sb_copy2d(host, host_pitch, view, (size_t)pitch, (size_t)w * 3, h, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-        rc = SB_ERR_CUDA;
-    if (cudaStreamSynchronize(s) != cudaSuccess && rc == SB_OK) rc = SB_ERR_CUDA;
-    gain_free(&gd, s);
-    if (rc == SB_ERR_CUDA) set_error("sb_gain_apply_dev: CUDA failure");
-    return rc;
+    return gain_apply(st, view, (long long)img->w * 3, w, h, host, host_pitch, gain_map, gw, gh, gc, gain_scalar);
 }
 
 int sb_timelapse_frame(const void *img, int is_s16, size_t pitch, const sb_devimg *dev, int dev_x, int dev_y, int w, int h, int tlx, int tly,
@@ -426,33 +240,20 @@ int sb_timelapse_frame(const void *img, int is_s16, size_t pitch, const sb_devim
         return SB_ERR_INVALID;
     }
     SB_TRY(ensure_device());
-    cudaStream_t s = default_stream();
-    Scratch tmp(s);
+    Staging st(default_stream());
     const int cw = roi[2], ch = roi[3];
-    uint8_t *d_dst = nullptr, *d_src = nullptr;
-    SB_TRY(tmp.get(&d_dst, (size_t)cw * 3 * ch));
-    const uint8_t *src8 = nullptr;
-    const int16_t *src16 = nullptr;
-    long long spitch = 0;
-    if (dev) {
-        src8 = dev->p + ((size_t)dev_y * dev->w + dev_x) * 3;
-        spitch = (long long)dev->w * 3;
-    } else {
-        // only the rows / columns that land on the canvas travel
-        SB_TRY(tmp.get(&d_src, (size_t)w * px * h));
-        SB_CUDA(sb_copy2d(d_src, (size_t)w * px, img, pitch, (size_t)w * px, h, cudaMemcpyHostToDevice, s));
-        if (is_s16) {
-            src16 = reinterpret_cast<const int16_t *>(d_src);
-            spitch = (long long)w * 3;
-        } else {
-            src8 = d_src;
-            spitch = (long long)w * 3;
-        }
-    }
-    SB_TRY(launch_timelapse_frame(src8, src16, spitch, w, h, tlx - roi[0], tly - roi[1], d_dst, (long long)cw * 3, cw, ch, s));
-    SB_CUDA(sb_copy2d(dst, dst_pitch, d_dst, (size_t)cw * 3, (size_t)cw * 3, ch, cudaMemcpyDeviceToHost, s));
-    SB_CUDA(cudaStreamSynchronize(s));
-    return SB_OK;
+    uint8_t *d_dst = st.tmp<uint8_t>((size_t)cw * 3 * ch);
+    // a device source is uint8; from the host, only the rows / columns that land on the canvas travel.  spitch: bytes of
+    // a uint8 row, elements of an int16 row
+    const bool s16 = is_s16 && !dev;
+    const uint8_t *src = dev ? dev->p + ((size_t)dev_y * dev->w + dev_x) * 3 : st.up<uint8_t>(img, pitch, (size_t)w * px, h);
+    const long long spitch = dev ? (long long)dev->w * 3 : (long long)w * 3;
+    st.run([&] {
+        return launch_timelapse_frame(s16 ? nullptr : src, s16 ? (const int16_t *)src : nullptr, spitch, w, h, tlx - roi[0], tly - roi[1],
+                                      d_dst, (long long)cw * 3, cw, ch, st.stream());
+    });
+    st.down(dst, dst_pitch, d_dst, (size_t)cw * 3, (size_t)cw * 3, ch);
+    return st.finish();
 }
 
 int sb_resize_exact(const uint8_t *src, size_t src_pitch, int sw, int sh, int channels, uint8_t *dst, size_t dst_pitch, int dw, int dh)
@@ -464,25 +265,17 @@ int sb_resize_exact(const uint8_t *src, size_t src_pitch, int sw, int sh, int ch
         return SB_ERR_INVALID;
     }
     SB_TRY(ensure_device());
-    cudaStream_t s = default_stream();
-    Scratch tmp(s);
-    uint8_t *d_src = nullptr, *d_dst = nullptr;
-    int *d_tx = nullptr, *d_ty = nullptr;
-    const size_t srow = (size_t)sw * channels, drow = (size_t)dw * channels;
-    SB_TRY(tmp.get(&d_src, srow * sh));
-    SB_TRY(tmp.get(&d_dst, drow * dh));
-    SB_TRY(tmp.get(&d_tx, (size_t)3 * dw));
-    SB_TRY(tmp.get(&d_ty, (size_t)3 * dh));
     std::vector<int> tx((size_t)3 * dw), ty((size_t)3 * dh);
     resize_exact_taps(sw, dw, tx.data());
     resize_exact_taps(sh, dh, ty.data());
-    SB_CUDA(sb_copy2d(d_src, srow, src, src_pitch, srow, sh, cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaMemcpyAsync(d_tx, tx.data(), tx.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    SB_CUDA(cudaMemcpyAsync(d_ty, ty.data(), ty.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    SB_TRY(launch_resize_exact(d_src, (long long)srow, channels, d_tx, d_ty, d_dst, (long long)drow, dw, dh, s));
-    SB_CUDA(sb_copy2d(dst, dst_pitch, d_dst, drow, drow, dh, cudaMemcpyDeviceToHost, s));
-    SB_CUDA(cudaStreamSynchronize(s));
-    return SB_OK;
+    Staging st(default_stream());
+    const size_t srow = (size_t)sw * channels, drow = (size_t)dw * channels;
+    const uint8_t *d_src = st.up<uint8_t>(src, src_pitch, srow, sh);
+    uint8_t *d_dst = st.tmp<uint8_t>(drow * dh);
+    const int *d_tx = st.up(tx), *d_ty = st.up(ty);
+    st.run([&] { return launch_resize_exact(d_src, (long long)srow, channels, d_tx, d_ty, d_dst, (long long)drow, dw, dh, st.stream()); });
+    st.down(dst, dst_pitch, d_dst, drow, drow, dh);
+    return st.finish();
 }
 
 int sb_seam_resize(const uint8_t *seam, size_t seam_pitch, int sw, int sh, const uint8_t *mask, size_t mask_pitch, int w, int h,
@@ -494,16 +287,12 @@ int sb_seam_resize(const uint8_t *seam, size_t seam_pitch, int sw, int sh, const
         return SB_ERR_INVALID;
     }
     SB_TRY(ensure_device());
-    cudaStream_t s = default_stream();
-    Scratch tmp(s);
-    uint8_t *d_mask = nullptr, *d_dst = nullptr;
-    SB_TRY(tmp.get(&d_mask, (size_t)w * h));
-    SB_TRY(tmp.get(&d_dst, (size_t)w * h));
-    SB_CUDA(sb_copy2d(d_mask, w, mask, mask_pitch, w, h, cudaMemcpyHostToDevice, s));
-    SB_TRY(seam_resize_device(seam, seam_pitch, sw, sh, d_mask, w, d_dst, w, w, h, s));
-    SB_CUDA(sb_copy2d(dst, dst_pitch, d_dst, w, w, h, cudaMemcpyDeviceToHost, s));
-    SB_CUDA(cudaStreamSynchronize(s));
-    return SB_OK;
+    Staging st(default_stream());
+    const uint8_t *d_mask = st.up<uint8_t>(mask, mask_pitch, w, h);
+    uint8_t *d_dst = st.tmp<uint8_t>((size_t)w * h);
+    st.run([&] { return seam_resize_device(seam, seam_pitch, sw, sh, d_mask, w, d_dst, w, w, h, st.stream()); });
+    st.down(dst, dst_pitch, d_dst, w, w, h);
+    return st.finish();
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -564,6 +353,7 @@ int sb_blender_num_bands(const sb_blender *b) { return b ? b->plan.nb : -1; }
 
 // one recorded feed: geometry first (host only, so that an out-of-roi feed fails before any device work), then the level-0
 // data on the device.  The image comes from the host (img) or from a device rectangle (dimg, dimg_pitch); likewise the mask.
+// A feed that fails leaves the blender as it was.
 static int blender_feed_impl(sb_blender *b, const void *img, int img_is_s16, size_t img_pitch, const uint8_t *dimg, size_t dimg_pitch,
                              const uint8_t *mask, size_t mask_pitch, const uint8_t *dmask, size_t dmask_pitch, int w, int h, int tl_x, int tl_y)
 {
@@ -572,58 +362,52 @@ static int blender_feed_impl(sb_blender *b, const void *img, int img_is_s16, siz
     f.w = w; f.h = h; f.tlx = tl_x; f.tly = tl_y;
     SB_TRY(b->plan.add_feed(f));
     FeedImage &im = b->plan.imgs.back();
-    const size_t px_bytes = img_is_s16 ? 6 : 3;
-    auto upload = [&]() -> int {
-        SB_TRY(ensure_device());
-        cudaStream_t s = default_stream();
-        const uint8_t *m_ptr = dmask;
-        size_t m_pitch = dmask_pitch;
-        if (!dmask) {
-            uint8_t *d_mask = nullptr;
-            SB_TRY(dev_alloc((void **)&d_mask, (size_t)w * h, s));
-            b->level0.push_back(d_mask);
-            SB_CUDA(sb_copy2d(d_mask, w, mask, mask_pitch, w, h, cudaMemcpyHostToDevice, s));
-            m_ptr = d_mask;
-            m_pitch = (size_t)w;
+    int rc = ensure_device();
+    if (rc == SB_OK) {
+        Staging st(default_stream());
+        cudaStream_t s = st.stream();
+        const size_t px_bytes = img_is_s16 ? 6 : 3;
+        const bool host_mask = !dmask;
+        // host images and masks are staged into buffers the blender keeps: from here on both sources are on the device
+        if (host_mask) {
+            uint8_t *d = st.keep<uint8_t>((size_t)w * h);
+            st.copy(d, w, mask, mask_pitch, w, h, cudaMemcpyHostToDevice);
+            dmask = d;
+            dmask_pitch = w;
         }
-        const uint8_t *i_ptr = dimg;
-        size_t i_pitch = dimg_pitch;
         if (!dimg) {
-            void *d_img = nullptr;
-            SB_TRY(dev_alloc(&d_img, (size_t)w * h * px_bytes, s));
-            b->level0.push_back(d_img);
-            SB_CUDA(sb_copy2d(d_img, (size_t)w * px_bytes, img, img_pitch, (size_t)w * px_bytes, h, cudaMemcpyHostToDevice, s));
-            i_ptr = (const uint8_t *)d_img;
-            i_pitch = (size_t)w * px_bytes;
+            uint8_t *d = st.keep<uint8_t>((size_t)w * h * px_bytes);
+            st.copy(d, (size_t)w * px_bytes, img, img_pitch, (size_t)w * px_bytes, h, cudaMemcpyHostToDevice);
+            dimg = d;
+            dimg_pitch = (size_t)w * px_bytes;
         }
         if (img_is_s16) {
-            if (dmask) {  // the generic layout keeps a pointer to the mask: it has to outlive this call
-                uint8_t *d_mask = nullptr;
-                SB_TRY(dev_alloc((void **)&d_mask, (size_t)w * h, s));
-                b->level0.push_back(d_mask);
-                SB_CUDA(sb_copy2d(d_mask, w, dmask, dmask_pitch, w, h, cudaMemcpyDeviceToDevice, s));
-                m_ptr = d_mask;
-                m_pitch = (size_t)w;
+            if (!host_mask) {  // the generic layout keeps a pointer to the mask: it has to outlive this call
+                uint8_t *d = st.keep<uint8_t>((size_t)w * h);
+                st.copy(d, w, dmask, dmask_pitch, w, h, cudaMemcpyDeviceToDevice);
+                dmask = d;
+                dmask_pitch = w;
             }
-            im.s16 = (const int16_t *)i_ptr;
+            im.s16 = (const int16_t *)dimg;
             im.s16_pitch = (long long)w * 3;
-            im.mask = m_ptr;
-            im.mask_pitch = (long long)m_pitch;
+            im.mask = dmask;
+            im.mask_pitch = (long long)dmask_pitch;
         } else {
-            uint32_t *d_rgbm = nullptr;
             const int rp = (w + 3) & ~3;  // 16-byte rows: the tile kernels stage windows of this buffer with 16-byte copies
-            SB_TRY(dev_alloc((void **)&d_rgbm, (size_t)rp * h * 4, s));
-            b->level0.push_back(d_rgbm);
-            if (rp != w) SB_CUDA(cudaMemsetAsync(d_rgbm, 0, (size_t)rp * h * 4, s));  // zero row padding = weight 0
-            SB_TRY(launch_pack_rgbm(i_ptr, (long long)i_pitch, m_ptr, (long long)m_pitch, d_rgbm, rp, w, h, s));
+            uint32_t *d_rgbm = st.keep<uint32_t>((size_t)rp * h);
+            if (rp != w)  // zero row padding = weight 0
+                st.run([&]() -> int {
+                    SB_CUDA(cudaMemsetAsync(d_rgbm, 0, (size_t)rp * h * 4, s));
+                    return SB_OK;
+                });
+            st.run([&] { return launch_pack_rgbm(dimg, (long long)dimg_pitch, dmask, (long long)dmask_pitch, d_rgbm, rp, w, h, s); });
             im.rgbm = d_rgbm;
             im.rgbm_pitch = rp;
         }
         // the caller's buffers (and device twins) may change as soon as we return
-        SB_CUDA(cudaStreamSynchronize(s));
-        return SB_OK;
-    };
-    const int rc = upload();
+        rc = st.finish();
+        if (rc == SB_OK) b->level0.insert(b->level0.end(), st.kept().begin(), st.kept().end());
+    }
     if (rc != SB_OK) b->plan.imgs.pop_back();
     return rc;
 }
@@ -683,35 +467,31 @@ int sb_blender_blend(sb_blender *b, uint8_t *dst, size_t dst_pitch, uint8_t *dst
         return SB_ERR_INVALID;
     }
     SB_TRY(ensure_device());
-    cudaStream_t s = default_stream();
-    Scratch tmp(s);
+    Staging st(default_stream());
+    cudaStream_t s = st.stream();
     PanoOut out;
     std::memset(&out, 0, sizeof out);
     out.w = w;
     out.h = h;
     if (dst) {
-        SB_TRY(tmp.get(&out.rgb, (size_t)w * 3 * h));
+        out.rgb = st.tmp<uint8_t>((size_t)w * 3 * h);
         out.rgb_pitch = (long long)w * 3;
     }
     if (dst_mask) {
-        SB_TRY(tmp.get(&out.mask, (size_t)w * h));
+        out.mask = st.tmp<uint8_t>((size_t)w * h);
         out.mask_pitch = w;
     }
     if (dst_s16) {
-        SB_TRY(tmp.get(&out.s16, (size_t)w * 3 * h));
+        out.s16 = st.tmp<int16_t>((size_t)w * 3 * h);
         out.s16_pitch = (long long)w * 3;
     }
-    int rc = b->plan.allocate(s);
-    if (rc == SB_OK) rc = b->plan.run(out, s);
-    if (rc == SB_OK) {  // (errors fall through to the clean-up below: the feeds are dropped either way)
-        cudaError_t e = cudaSuccess;
-        if (dst) e = sb_copy2d(dst, dst_pitch, out.rgb, (size_t)w * 3, (size_t)w * 3, h, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess && dst_mask) e = sb_copy2d(dst_mask, mask_pitch, out.mask, w, w, h, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess && dst_s16) e = sb_copy2d(dst_s16, s16_pitch, out.s16, (size_t)w * 6, (size_t)w * 6, h, cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) rc = cuda_fail(e, "sb_blender_blend: copy of the result", __FILE__, __LINE__);
-    }
-    // like OpenCV, blend() consumes the state: a new prepare() is needed before the next feed
+    st.run([&] { return b->plan.allocate(s); });
+    st.run([&] { return b->plan.run(out, s); });
+    if (dst) st.down(dst, dst_pitch, out.rgb, (size_t)w * 3, (size_t)w * 3, h);
+    if (dst_mask) st.down(dst_mask, mask_pitch, out.mask, w, w, h);
+    if (dst_s16) st.down(dst_s16, s16_pitch, out.s16, (size_t)w * 6, (size_t)w * 6, h);
+    const int rc = st.finish();
+    // like OpenCV, blend() consumes the state, also when it fails: a new prepare() is needed before the next feed
     blender_drop_feeds(b);
     b->prepared = false;
     return rc;

@@ -119,21 +119,16 @@ int comm_allgather_bytes(const void *mine, void *all, size_t bytes_per_rank, cud
         set_error("NCCL library lacks ncclAllGather");
         return SB_ERR_COMM;
     }
-    void *d_in = nullptr, *d_out = nullptr;
-    SB_TRY(dev_alloc(&d_in, bytes_per_rank, s));
-    SB_TRY(dev_alloc(&d_out, bytes_per_rank * (size_t)g_world, s));
-    int rc = SB_OK;
-    if (cudaMemcpyAsync(d_in, mine, bytes_per_rank, cudaMemcpyHostToDevice, s) != cudaSuccess) rc = SB_ERR_CUDA;
-    if (rc == SB_OK) {
+    const size_t all_bytes = bytes_per_rank * (size_t)g_world;
+    Staging st(s);
+    uint8_t *d_in = st.tmp<uint8_t>(bytes_per_rank), *d_out = st.tmp<uint8_t>(all_bytes);
+    st.copy(d_in, bytes_per_rank, mine, bytes_per_rank, bytes_per_rank, 1, cudaMemcpyHostToDevice);
+    st.run([&] {
         const int nrc = p_allgather(d_in, d_out, bytes_per_rank, 0 /* ncclChar */, g_comm, s);
-        if (nrc) rc = nccl_fail(nrc, "ncclAllGather");
-    }
-    if (rc == SB_OK && cudaMemcpyAsync(all, d_out, bytes_per_rank * (size_t)g_world, cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = SB_ERR_CUDA;
-    if (cudaStreamSynchronize(s) != cudaSuccess && rc == SB_OK) rc = SB_ERR_CUDA;
-    dev_free(d_in, s);
-    dev_free(d_out, s);
-    if (rc == SB_ERR_CUDA) set_error("comm_allgather_bytes: CUDA failure");
-    return rc;
+        return nrc ? nccl_fail(nrc, "ncclAllGather") : SB_OK;
+    });
+    st.down(all, all_bytes, d_out, all_bytes, all_bytes, 1);
+    return st.finish();
 }
 }  // namespace sb
 

@@ -16,9 +16,6 @@
 
 namespace sb {
 inline int rgbm_pitch_of(int w) { return (w + 31) & ~31; }
-
-int make_warp_job(const Projector &p, const int rect[4], int src_w, int src_h, float *tab_dev, WarpJob *job, cudaStream_t s,
-                  std::vector<float> &host_tab);
 }
 using namespace sb;
 
@@ -1064,13 +1061,15 @@ int sb_compositor_time_multi(sb_compositor *const *cs, int n, int iters, float *
     for (int it = 0; it < iters && rc == SB_OK; ++it) rc = compositor_enqueue(cs[it % n], false);
     float worst = 0.f;
     for (int k = 0; k < n; ++k) {
-        if (cudaEventRecord(ends[k], cs[k]->stream) != cudaSuccess || cudaEventSynchronize(ends[k]) != cudaSuccess) rc = rc == SB_OK ? SB_ERR_CUDA : rc;
+        cudaError_t e = cudaEventRecord(ends[k], cs[k]->stream);
+        if (e != cudaSuccess && rc == SB_OK) rc = cuda_fail(e, "cudaEventRecord", __FILE__, __LINE__);
+        if (e == cudaSuccess && (e = cudaEventSynchronize(ends[k])) != cudaSuccess && rc == SB_OK)
+            rc = cuda_fail(e, "cudaEventSynchronize", __FILE__, __LINE__);
         float t = 0.f;
         if (rc == SB_OK && cudaEventElapsedTime(&t, start, ends[k]) == cudaSuccess) worst = t > worst ? t : worst;
     }
     (void)cudaEventDestroy(start);
     for (int k = 0; k < n; ++k) (void)cudaEventDestroy(ends[k]);
-    if (rc != SB_OK && rc == SB_ERR_CUDA) set_error("sb_compositor_time_multi: CUDA failure while timing");
     *ms_total = worst;
     return rc;
 }

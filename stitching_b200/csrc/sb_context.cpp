@@ -107,6 +107,39 @@ void dev_free(void *p, cudaStream_t s)
     if (p) (void)cudaFreeAsync(p, s);
 }
 
+void *Staging::alloc(size_t bytes, std::vector<void *> &list)
+{
+    void *p = nullptr;
+    if (rc_ == SB_OK) rc_ = dev_alloc(&p, bytes, s_);
+    if (p) list.push_back(p);
+    return p;
+}
+
+void Staging::copy(void *dst, size_t dpitch, const void *src, size_t spitch, size_t width, size_t rows, cudaMemcpyKind kind)
+{
+    if (rc_ != SB_OK) return;
+    const cudaError_t e = sb_copy2d(dst, dpitch, src, spitch, width, rows, kind, s_);
+    if (e != cudaSuccess) rc_ = cuda_fail(e, dpitch == width && spitch == width ? "cudaMemcpyAsync" : "cudaMemcpy2DAsync", __FILE__, __LINE__);
+}
+
+int Staging::finish()
+{
+    if (!finished_) {
+        finished_ = true;
+        const cudaError_t e = cudaStreamSynchronize(s_);
+        if (e != cudaSuccess && rc_ == SB_OK) rc_ = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
+    }
+    return rc_;
+}
+
+Staging::~Staging()
+{
+    finish();
+    for (void *p : tmps_) dev_free(p, s_);
+    if (rc_ != SB_OK)
+        for (void *p : kept_) dev_free(p, s_);
+}
+
 }  // namespace sb
 
 extern "C" {
@@ -152,14 +185,14 @@ int sb_selftest_division(unsigned long long n, unsigned long long seed, int mode
         sb::set_error("sb_selftest_division: bad arguments");
         return SB_ERR_INVALID;
     }
-    unsigned long long *bad = nullptr;
-    SB_TRY(sb::dev_alloc((void **)&bad, sizeof *bad, sb::g_stream));
-    SB_CUDA(cudaMemsetAsync(bad, 0, sizeof *bad, sb::g_stream));
-    int rc = sb::launch_selftest_division(n, seed, mode, bad, sb::g_stream);
-    if (rc == SB_OK && cudaMemcpyAsync(mismatches, bad, sizeof *bad, cudaMemcpyDeviceToHost, sb::g_stream) != cudaSuccess) rc = SB_ERR_CUDA;
-    if (rc == SB_OK && cudaStreamSynchronize(sb::g_stream) != cudaSuccess) rc = SB_ERR_CUDA;
-    sb::dev_free(bad, sb::g_stream);
-    return rc;
+    sb::Staging st(sb::g_stream);
+    unsigned long long *bad = st.tmp<unsigned long long>(1);
+    st.run([&] {
+        SB_CUDA(cudaMemsetAsync(bad, 0, sizeof *bad, sb::g_stream));
+        return sb::launch_selftest_division(n, seed, mode, bad, sb::g_stream);
+    });
+    st.down(mismatches, sizeof *bad, bad, sizeof *bad, sizeof *bad, 1);
+    return st.finish();
 }
 
 void *sb_host_alloc(size_t bytes)

@@ -45,6 +45,55 @@ cudaError_t host_alloc_pinned(void **p, size_t bytes);
 int dev_alloc(void **p, size_t bytes, cudaStream_t s);
 void dev_free(void *p, cudaStream_t s);
 
+// The device work of one call that reads or writes its caller's memory, on stream `s` (sb_context.cpp).  It keeps the
+// temporaries, the buffers that outlive a successful call and the first failure; once a step has failed every later one is
+// skipped (allocations return null).  finish() synchronises `s` on every path, so that no copy from or to the caller's
+// memory is still in flight, and returns the first failure; the destructor does the same if finish() was not called, then
+// frees the temporaries, and the kept buffers too when a step failed.
+class Staging {
+  public:
+    explicit Staging(cudaStream_t s) : s_(s) {}
+    ~Staging();
+    Staging(const Staging &) = delete;
+    Staging &operator=(const Staging &) = delete;
+    cudaStream_t stream() const { return s_; }
+    // a step that returns SB_OK or a failure whose message it has set
+    template <typename F>
+    void run(F &&step)
+    {
+        if (rc_ == SB_OK) rc_ = step();
+    }
+    template <typename T>
+    T *tmp(size_t count) { return (T *)alloc(count * sizeof(T), tmps_); }
+    template <typename T>
+    T *keep(size_t count) { return (T *)alloc(count * sizeof(T), kept_); }
+    const std::vector<void *> &kept() const { return kept_; }
+    // `rows` rows of `width` bytes (row pitch `pitch`) between two buffers, as sb_copy2d
+    void copy(void *dst, size_t dpitch, const void *src, size_t spitch, size_t width, size_t rows, cudaMemcpyKind kind);
+    // a host rectangle into a new temporary of `rows` rows of `width` bytes
+    template <typename T>
+    T *up(const void *src, size_t pitch, size_t width, size_t rows)
+    {
+        T *d = (T *)alloc(width * rows, tmps_);
+        copy(d, width, src, pitch, width, rows, cudaMemcpyHostToDevice);
+        return d;
+    }
+    template <typename T>
+    T *up(const std::vector<T> &v) { return up<T>(v.data(), v.size() * sizeof(T), v.size() * sizeof(T), 1); }
+    void down(void *dst, size_t dpitch, const void *src, size_t spitch, size_t width, size_t rows)
+    {
+        copy(dst, dpitch, src, spitch, width, rows, cudaMemcpyDeviceToHost);
+    }
+    int finish();
+
+  private:
+    void *alloc(size_t bytes, std::vector<void *> &list);
+    cudaStream_t s_;
+    int rc_ = SB_OK;
+    bool finished_ = false;
+    std::vector<void *> tmps_, kept_;
+};
+
 // ---------------------------------------------------------------------------------------------
 // geometry (host, libm): sb_geometry.cpp
 // ---------------------------------------------------------------------------------------------
@@ -218,7 +267,11 @@ bool collapse_tile_enabled();
 // jobs are HOST structs: they are passed by value in the kernel parameter block, SB_WARP_BATCH images per launch
 #define SB_WARP_BATCH 32
 int launch_warp(const WarpJob *jobs_host, int n_jobs, cudaStream_t s);
-int warp_maps_upload(const Projector &p, const int rect[4], float *maps_dev, WarpJob *job, cudaStream_t s);  // sb_api.cpp
+// the device tables (`tab_dev`, warp_table_floats(w, h)) and the job of one image warped to `rect`; the upload reads
+// `host_tab` until `s` is synchronised (sb_jobs.cpp)
+int make_warp_job(const Projector &p, const int rect[4], int src_w, int src_h, float *tab_dev, WarpJob *job, cudaStream_t s,
+                  std::vector<float> &host_tab);
+int warp_maps_upload(const Projector &p, const int rect[4], float *maps_dev, WarpJob *job, cudaStream_t s);  // sb_jobs.cpp
 // u8x3 contiguous (w * h pixels) -> r | g<<8 | b<<16 words (the compositor's source layout for the warp kernel)
 int launch_repack_rgbx(const uint8_t *rgb, uint32_t *dst, long long pixels, cudaStream_t s);
 // launch_warp's kernel choice for a batch of jobs: true when it reads WarpJob::src4 of jobs that have one (sb_warp.cu)

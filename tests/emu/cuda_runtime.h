@@ -10,6 +10,7 @@
 // measured or shipped runs through it.
 #pragma once
 #include <cmath>
+#include <atomic>
 #include <condition_variable>
 #include <cstdint>
 #include <cstdlib>
@@ -19,7 +20,7 @@
 #include <vector>
 
 typedef int cudaError_t;
-enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2 };
+enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2, cudaErrorUnknown = 999 };
 typedef struct emuStream_st *cudaStream_t;
 typedef struct emuEvent_st *cudaEvent_t;
 typedef int cudaMemPool_t;
@@ -60,14 +61,28 @@ static inline unsigned __vmins2(unsigned a, unsigned b)
     return emu_lanes2(emu_lo16(a) < emu_lo16(b) ? emu_lo16(a) : emu_lo16(b), emu_hi16(a) < emu_hi16(b) ? emu_hi16(a) : emu_hi16(b));
 }
 
-static inline const char *cudaGetErrorString(cudaError_t) { return "emu"; }
-static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
+// sb_emu_fail_at(k) (emu_globals.cpp): the k-th fallible runtime call from then on fails -- cudaMallocAsync with
+// cudaErrorMemoryAllocation; cudaMemcpyAsync, cudaMemcpy2DAsync, cudaStreamSynchronize and cudaGetLastError (the launch
+// checks) with cudaErrorUnknown -- and the hook disarms; k = 0 disarms it.  sb_emu_live_allocs(): live cudaMallocAsync blocks
+extern std::atomic<int> emu_fail_in;
+extern std::atomic<long> emu_live_allocs;
+static inline bool emu_fails()
+{
+    int k = emu_fail_in.load();
+    while (k > 0 && !emu_fail_in.compare_exchange_weak(k, k - 1)) {}
+    return k == 1;
+}
+static inline const char *cudaGetErrorString(cudaError_t e)
+{
+    return e == cudaErrorMemoryAllocation ? "out of memory" : e == cudaErrorUnknown ? "unknown error" : "emu";
+}
+static inline cudaError_t cudaGetLastError() { return emu_fails() ? cudaErrorUnknown : cudaSuccess; }
 static inline cudaError_t cudaGetDeviceCount(int *n) { *n = 8; return cudaSuccess; }
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { std::memset(p, 0, sizeof *p); std::strcpy(p->name, "EMU (tests only)"); p->major = 9; p->multiProcessorCount = 132; return cudaSuccess; }
 static inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, unsigned) { *s = (cudaStream_t)std::malloc(1); return cudaSuccess; }
 static inline cudaError_t cudaStreamDestroy(cudaStream_t s) { std::free(s); return cudaSuccess; }
-static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
+static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return emu_fails() ? cudaErrorUnknown : cudaSuccess; }
 static inline cudaError_t cudaDeviceGetDefaultMemPool(cudaMemPool_t *p, int) { *p = 0; return cudaSuccess; }
 static inline cudaError_t cudaMemPoolSetAttribute(cudaMemPool_t, cudaMemPoolAttr, void *) { return cudaSuccess; }
 // SB_EMU_FILL=<byte> (e.g. 0xff): every new device and page-locked allocation starts filled with that byte instead of
@@ -79,14 +94,31 @@ static inline void *emu_alloc(size_t n)
     if (p && fill && *fill) std::memset(p, (int)(std::strtol(fill, nullptr, 0) & 0xff), n);
     return p;
 }
-static inline cudaError_t cudaMallocAsync(void **p, size_t n, cudaStream_t) { *p = emu_alloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
-static inline cudaError_t cudaFreeAsync(void *p, cudaStream_t) { std::free(p); return cudaSuccess; }
+static inline cudaError_t cudaMallocAsync(void **p, size_t n, cudaStream_t)
+{
+    *p = emu_fails() ? nullptr : emu_alloc(n);
+    if (!*p) return cudaErrorMemoryAllocation;
+    ++emu_live_allocs;
+    return cudaSuccess;
+}
+static inline cudaError_t cudaFreeAsync(void *p, cudaStream_t)
+{
+    if (p) --emu_live_allocs;
+    std::free(p);
+    return cudaSuccess;
+}
 static inline cudaError_t cudaMallocHost(void **p, size_t n) { *p = emu_alloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 static inline cudaError_t cudaFreeHost(void *p) { std::free(p); return cudaSuccess; }
 static inline cudaError_t cudaMemsetAsync(void *d, int v, size_t n, cudaStream_t) { std::memset(d, v, n); return cudaSuccess; }
-static inline cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, cudaMemcpyKind, cudaStream_t) { std::memcpy(d, s, n); return cudaSuccess; }
+static inline cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, cudaMemcpyKind, cudaStream_t)
+{
+    if (emu_fails()) return cudaErrorUnknown;
+    std::memcpy(d, s, n);
+    return cudaSuccess;
+}
 static inline cudaError_t cudaMemcpy2DAsync(void *d, size_t dp, const void *s, size_t sp, size_t w, size_t h, cudaMemcpyKind, cudaStream_t)
 {
+    if (emu_fails()) return cudaErrorUnknown;
     for (size_t y = 0; y < h; ++y) std::memcpy((char *)d + y * dp, (const char *)s + y * sp, w);
     return cudaSuccess;
 }

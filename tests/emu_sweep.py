@@ -33,6 +33,7 @@ def corpora(L, O):
     import test_final_scale
     import test_fullres
     import test_gain_maps as GT
+    import test_host_entries as HE
     import test_host_logic as H
     import test_shard_fuzz
     import test_timelapse_compositor as TL
@@ -77,11 +78,12 @@ def corpora(L, O):
            ("timelapse", lambda mp: GT.test_timelapse_with_clipped_parts(L, O)),
            ("sharded", lambda mp: GT.test_sharded_owner_sets_the_gain(L, O))]
         + [(f"compositor_{k}", lambda mp, k=k: GT.test_compositor_set_gain(L, O, k)) for k in (3, 4)],
+        "host_entries": [(f"{fn.__name__}[{a}]", lambda mp, fn=fn, a=a: fn(HE.hooked(L), *a)) for fn, a in HE.cases()],
     }
 
 
 NAMES = ["rig_fuzz", "crop_fuzz", "shard_fuzz", "dropin_fuzz", "final_scale", "timelapse_fuzz", "fullres", "goldens",
-         "setters", "lanes_blocks", "kernel_edges", "gain_maps"]
+         "setters", "lanes_blocks", "kernel_edges", "gain_maps", "host_entries"]
 
 
 def run(lib_path, names, out=sys.stdout, only=None):

@@ -152,7 +152,7 @@ CATALOGUE = [
     M("gain_ipp_unfused", "sb_warp.cu", "const float h0 = fmaf(fadd(b0, -a0), fx, a0), h1",
       "const float h0 = fadd(fmul(fadd(b0, -a0), fx), a0), h1",
       "apply_gain: the IPP tap of a map with both sides >= 2 rounded twice instead of fused", ["gain_maps:apply_ipp"], "rounding"),
-    M("gain_dispatch_and", "sb_api.cpp", "const bool generic = gw == 1 || gh == 1;", "const bool generic = gw == 1 && gh == 1;",
+    M("jobs_gain_dispatch_and", "sb_jobs.cpp", "const bool generic = gw == 1 || gh == 1;", "const bool generic = gw == 1 && gh == 1;",
       "gain_upload: a 1 x k or k x 1 map takes IPP's taps and passes (only 1 x 1 takes OpenCV's own)", ["gain_maps:timelapse"], "predicate"),
     M("gain_rows_zeroed", "sb_geometry.cpp", "if (form == TAPS_COLS && (s < 0", "if (form != TAPS_IPP && (s < 0",
       "resize_f32_taps: the rows of a map with a side of 1 zero the fraction at the clamped ends, as IPP does", ["gain_maps:compositor_3"],
